@@ -2,14 +2,16 @@
 """Benchmark of the parallel-denoising hot path (BASELINE.json metric):
 denoised tokens/sec (text+image) per 512x512 @ 64-step sample, variant A 8B, cfg_img=4 (BASELINE configs[1]).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W]            # this repo's CUDA path
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR] [--profile] [--extras] [--cpu-baseline]
     python bench.py --impl reference ...                            # the reference algorithm on the host CPU (oracle port)
 
 One "step" = one full sample = one generate_ti2ti call: 128 denoising iterations, 192 transformer forwards
 (128 conditional + 64 unconditional-image), 128 text steps, 64 image steps -> 1280 denoised tokens.
 Under torchrun (N > 1) every rank denoises its own independent prompt (replicas, no data-path collective): weak scaling.
 Prints ONE JSON line on rank 0. Timing: CUDA events on the launching stream, barrier + synchronize on both sides,
-max over ranks. Weights (16.2 GB) are re-read from HBM every forward, far beyond the 126 MB L2, so no L2 flush is needed.
+max over ranks. Weights (16.2 GB) are re-read from HBM every forward, far beyond the 50 MB L2 of an H100, so no L2 flush is
+needed. --dump-outputs DIR writes the id buffer the last timed sample produced (float64 .npy) for output-for-output
+comparisons between builds: weights, prompt and noise are seeded, so the same arguments give the same inputs.
 """
 from __future__ import annotations
 
@@ -69,6 +71,16 @@ def quiet():
 # ------------------------------------------------------------------------------------------------------------------
 # clocks
 # ------------------------------------------------------------------------------------------------------------------
+def _die_with_parent():
+    """Child-process hook: the sampler is killed with the benchmark even when the benchmark itself is killed (Linux prctl)."""
+    import ctypes
+    import signal
+    try:
+        ctypes.CDLL("libc.so.6", use_errno=True).prctl(1, signal.SIGTERM)  # PR_SET_PDEATHSIG
+    except OSError:
+        pass
+
+
 class ClockSampler:
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -80,7 +92,7 @@ class ClockSampler:
         try:
             self.f = open(self.path, "w")
             self.p = subprocess.Popen(["nvidia-smi", f"--query-gpu={self.Q}", "--format=csv,noheader,nounits", "-lms", "200",
-                                       "-i", str(self.idx)], stdout=self.f, stderr=subprocess.DEVNULL)
+                                       "-i", str(self.idx)], stdout=self.f, stderr=subprocess.DEVNULL, preexec_fn=_die_with_parent)
         except Exception:
             self.p = None
 
@@ -139,7 +151,7 @@ def host_cpu_info():
 
 
 def cpu_reference_sample(model_cfg: dict, reps: int = 3):
-    """Times the path's CPU restatement (oracle/, the port of the reference; /root/reference is not on the GPU box) at
+    """Times the path's CPU restatement (oracle/, the port of the reference; the benchmark does not depend on the reference) at
     the full BASELINE shapes on a bounded sample and extrapolates to one full sample with the exact operation counts:
       192 forwards x n_layers block-forwards  +  128 text-row heads  +  128 image-col heads (64 cond + 64 uncond)
       + 128 text steps + 64 image steps.
@@ -211,7 +223,7 @@ def cpu_reference_sample(model_cfg: dict, reps: int = 3):
 def gpu_eager_baseline(model_cfg: dict, device: str, lay: dict, seed: int = 1000):
     """The reference ALGORITHM in PyTorch eager on this GPU (BASELINE.md 4(iii), SURVEY 8d "the practical bar to beat"):
     the oracle port of LLaDAModel.forward + the generate_ti2ti step run with device='cuda' tensors - cuBLAS GEMMs, torch SDPA,
-    ATen elementwise kernels, FULL LM head [L, V] like the reference. /root/reference itself is not on the GPU box, so the
+    ATen elementwise kernels, FULL LM head [L, V] like the reference. The benchmark does not depend on the reference itself, so the
     port stands in for it, which FAVOURS the baseline: its step has none of the reference's ~3 300 .item() syncs per image
     step and it skips the unused uncond_text forward. Timed: 4 text-only steps and 2 image steps (cond + uncond_image
     forwards) after one warm-up of each, extrapolated with the exact counts of the workload (64 + 64)."""
@@ -303,11 +315,11 @@ def workload_config(args, n_gpus):
             "seq_len": 2414, "forwards_per_sample": 192,
             "parallelism": (f"tensor-parallel x{n_gpus} (one prompt; heads/ff/vocab split, " + ("fused reduce+residual+norm+broadcast kernel over NVLink peer memory)" if getattr(args, "tp_collective", "p2p") == "p2p" else "fp32 all-reduce over NCCL)") if getattr(args, "tp", False) and n_gpus > 1
                             else f"replicas x{n_gpus} (independent prompts, no collective)"),
-            "weights": "synthetic normal(0, 0.02) bf16, seeded", "l2": "16.2 GB of weights streamed per forward >> 126 MB L2 (no flush needed)"}
+            "weights": "synthetic normal(0, 0.02) bf16, seeded", "l2": "16.2 GB of weights streamed per forward >> 50 MB L2 (no flush needed)"}
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ------------------------------------------------------------------------------------------------------------------
 def model_namespace(model_cfg: dict):
     from types import SimpleNamespace
@@ -438,14 +450,14 @@ def measure_variant_m(args, rank: int, world: int, device: str, steps: int, warm
            "ms_per_step": ms / steps, "scaling": "weak",
            "config": {"workload": "MMaDA-Parallel-M 8B (BASELINE configs[4] shape per GPU): 1 prompt per GPU, L=2341, CFG batch 2 on each of 128 "
                                   "steps, 64 image steps, text_cfg=2.5, image_cfg=4.0", "parallelism": f"replicas x{world} (no collective)",
-                      "gemm_kernel": "cta_group::2 pair kernel (M = 4682: 19 pair m-tiles; the default for M > 256, MMDP_GEMM_PAIR=0 routes the 1-CTA kernel)"},
+                      "gemm_kernel": "persistent wgmma kernel, 128 x 256 tiles (M = 4682: 37 m-tiles)"},
            "e2e": {"value": v, "unit": "tokens/s", "h2d_bytes_per_step": int(inp.numel() * 16), "d2h_bytes_per_step": 256 * 8},
            "algorithmic_pflop_per_sample": flops / 1e15,
            "whole_step_tflops_per_gpu": flops * steps / (ms / 1e3) / 1e12}
     if prof is not None:
         peaks = load_peaks()
         gm, gf, gn = prof["gemm"]
-        rec["roofline"] = {"kernel": "gemm_pair_kernel / gemm_bf16_kernel (tcgen05, all epilogues)", "bound": "tensor", "achieved": gf / (gm / 1e3) / 1e12 if gm else None,
+        rec["roofline"] = {"kernel": "gemm_bf16_kernel (wgmma, all epilogues)", "bound": "tensor", "achieved": gf / (gm / 1e3) / 1e12 if gm else None,
                            "peak": peaks[0], "unit": "TFLOP/s", "frac": (gf / (gm / 1e3) / 1e12 / peaks[0]) if gm else None, "peak_source": peaks[1],
                            "launches": gn, "avg_launch_ms": gm / max(1, gn)}
         rec["kernel_breakdown_one_sample_ms"] = {"gemm": gm, "attention": prof["attention"][0], "row_kernels": prof["row"][0], "sampling": prof["sampling"][0],
@@ -471,9 +483,9 @@ def run_variant_m(args, rank, local_rank, world):
 def load_peaks():
     try:
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        return peaks.get("bf16_tflops_sustained", 1400.0), "MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)", peaks
+        return peaks.get("bf16_tflops_sustained", 989.0), "MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)", peaks
     except Exception:
-        return 1400.0, "fallback ~1.4 PFLOP/s sustained (B200_PROFILING.md)", {}
+        return 989.0, "NVIDIA H100 SXM data sheet: 989 TFLOP/s dense BF16 at up to 700 W (not a measured rate)", {}
 
 
 def measure_vq_decode(device: str, iters: int = 10):
@@ -511,14 +523,14 @@ def measure_vq_decode(device: str, iters: int = 10):
     rm, rb, rn = prof["row"]
     return {"ms_per_image": ms, "image": "1024 ids -> 3x512x512 fp32", "conv_tf32_ms": cm, "conv_tf32_launches": cn,
             "conv_tf32_tflops": cf / (cm / 1e3) / 1e12 if cm else None, "conv_flops_per_image": cf,
-            "tf32_peak_nominal_tflops": 1100.0, "frac_of_nominal_tf32": (cf / (cm / 1e3) / 1e12 / 1100.0) if cm else None,
+            "tf32_peak_nominal_tflops": 495.0, "frac_of_nominal_tf32": (cf / (cm / 1e3) / 1e12 / 495.0) if cm else None,
             "row_kernels_ms": rm, "row_kernels_GBps": rb / (rm / 1e3) / 1e9 if rm else None,
             "preview_path_cost_ms": 38 * ms, "note": "the step-wise preview loop (A/app.py) decodes after each of its 38 image steps"}
 
 
 def measure_tensor_parallel(args, model_cfg, device, rank, world, replica_model, steps: int):
     """BASELINE configs[3]: ONE sample tensor-parallel over the `world` GPUs (strong scaling). Runs on every rank; includes a
-    parity self-check the driver's multi-GPU lease can see: logits of the TP forward against the single-GPU forward of the
+    parity self-check in the benchmark record: logits of the TP forward against the single-GPU forward of the
     same (seed-1000) weights, and the ranks' final ids compared."""
     import torch.distributed as dist
     from mmada_parallel_b200.generators.parallel_generator import DenoiseState, denoise_loop
@@ -532,13 +544,14 @@ def measure_tensor_parallel(args, model_cfg, device, rank, world, replica_model,
         from mmada_parallel_b200 import _lib
         a_tp, _ = tp.forward_rows(ids, rows_a=text_rows)
         a_1, _ = replica_model.forward_rows(ids, rows_a=text_rows)
-        # yardstick: the same single-GPU forward with the other GEMM kernel (1-CTA tiles + split-K tail instead of CTA pairs) -
-        # another valid accumulation order. A 32-layer random-weight network amplifies 1-ulp differences, so the bound for
-        # the TP forward is "as close to the single-GPU forward as two single-GPU schedules are to each other" (x1.5);
-        # the strict 4-ulp bound is enforced on the 2-layer model in tests/test_gpu_tp.py.
-        _lib.lib.mmdp_set_gemm_pair(0)
+        # yardstick: the same single-GPU forward with the other GEMM schedule (split-K tails wherever a partial wave exists
+        # instead of where the cost model says they pay) - another valid accumulation order. A 32-layer random-weight network
+        # amplifies 1-ulp differences, so the bound for the TP forward is "as close to the single-GPU forward as two
+        # single-GPU schedules are to each other" (x1.5); the strict 4-ulp bound is enforced on the 2-layer model in
+        # tests/test_gpu_tp.py.
+        _lib.lib.mmdp_set_gemm_splitk(3)
         a_alt, _ = replica_model.forward_rows(ids, rows_a=text_rows)
-        _lib.lib.mmdp_set_gemm_pair(1)
+        _lib.lib.mmdp_set_gemm_splitk(2)
         scale = a_1.float().abs().max().item()
         err = (a_tp.float() - a_1.float()).abs()
         max_ulp = err.max().item() / (scale * 2.0 ** -8)
@@ -587,7 +600,7 @@ def measure_tensor_parallel(args, model_cfg, device, rank, world, replica_model,
         # 2 chunks on two streams: one chunk's NVLink traffic under the other's GEMMs), one sample
         one_chunk_tok_s = None
         main_chunks = int(getattr(tp, "chunks", 1))
-        if getattr(args, "tp_alt_schedule", False):  # opt-in: its numbers are on record (profiles/r02), the default run stays minimal
+        if getattr(args, "tp_alt_schedule", False):  # opt-in: the default run stays minimal
             tp.chunks, tp._ctx_key = (1 if main_chunks == 2 else 2), None
             dist.barrier()
             torch.cuda.synchronize()
@@ -636,7 +649,20 @@ def measure_tensor_parallel(args, model_cfg, device, rank, world, replica_model,
                           "text_row_argmax_agreement": argmax_equal, "yardstick_argmax_agreement": argmax_yard,
                           "ranks_final_ids_identical": bool(int(same.item()) == 1),
                           "against": "single-GPU forward of the same 32-layer weights on this rank (256 text rows x V); yardstick = the same "
-                                     "single-GPU forward with the 1-CTA GEMM kernel instead of the CTA-pair kernel"}}
+                                     "single-GPU forward with split-K tails on every partial wave"}}
+
+
+def dump_outputs(out_dir: str, ids: torch.Tensor, lay: dict):
+    """What a caller of the timed path receives from its last sample: the whole id buffer [L], and the generated text ids
+    and image VQ ids cut out of it (the image grid rows without their newline tokens). int64 ids as float64 (exact)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    ids = ids.reshape(-1).cpu()
+    grid, start = lay["newline_every"], lay["image_start"]
+    img_pos = torch.tensor([start + r * (grid + 1) + c for r in range(lay["seq_len"] // grid) for c in range(grid)])
+    arrays = {"ids": ids, "text_ids": ids[lay["text_start"]:lay["text_end"]], "image_ids": ids[img_pos]}
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.to(torch.float64).numpy())
 
 
 def main():
@@ -644,10 +670,15 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=2)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--impl", default="b200", choices=["b200", "reference"], help="b200 = this repo's CUDA path (the name is historical)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the id buffer of the last timed sample to DIR/*.npy")
     ap.add_argument("--tiny", action="store_true", help="2-layer d=256 model: plumbing check only (INVALID as a benchmark number)")
-    ap.add_argument("--no-cpu-baseline", action="store_true")
-    ap.add_argument("--no-extras", action="store_true", help="skip the sub-records (tensor-parallel at N > 1, variant M, torch-eager GPU "
+    # The sub-records take longer than the contract line itself on an H100 (the CPU port alone runs minutes of full-shape block
+    # forwards), so they are opt-in: the default run is the timed samples, the e2e pass and the one profiled sample.
+    ap.add_argument("--cpu-baseline", action="store_true", help="also time the reference algorithm on the host CPU (minutes)")
+    ap.add_argument("--profile", action="store_true", help="also run one sample with every launch timed by CUDA events (roofline and "
+                    "kernel breakdown records)")
+    ap.add_argument("--extras", action="store_true", help="also run the sub-records (tensor-parallel at N > 1, variant M, torch-eager GPU "
                     "baseline, VQ decode timing)")
     ap.add_argument("--variant", default="a", choices=["a", "m"], help="a = BASELINE configs[1] (the contract metric); m = extra line for "
                     "variant M (interleave_generate, CFG batch 2 every step, BASELINE configs[4] per GPU)")
@@ -717,19 +748,23 @@ def main():
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record()
         for st in states:
-            denoise_loop(st, generator=rng, **loop_kw)
+            last_ids = denoise_loop(st, generator=rng, **loop_kw)
         ev1.record()
         barrier()
         launches = int(_lib.lib.mmdp_launch_count(0))
         clock_info = clocks.stop() if rank == 0 else None
         ms_value = max_over_ranks(ev0.elapsed_time(ev1), device=device)
+        if args.dump_outputs and rank == 0 and args.steps > 0:
+            dump_outputs(args.dump_outputs, last_ids, lay)
 
-        # ---- timed region 2: through the public API with HOST buffers ("e2e"): H2D of the inputs + D2H of the result inside
+        # ---- timed region 2: ONE sample through the public API with HOST buffers ("e2e"): H2D of the inputs + D2H of the result
+        # inside. One sample: it differs from region 1 only by the copies, and a second K-sample pass would double the run time.
+        e2e_steps = 1 if args.steps > 0 else 0
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         with quiet():
-            for _ in range(args.steps):
+            for _ in range(e2e_steps):
                 img, txt = generate_ti2ti(model, host_ids, uncon_text=lay["uncon_text"], uncon_image=lay["uncon_image"], generator=rng,
                                           text_gen_length=gen["text_gen_length"], text_block_length=gen["text_block_length"],
                                           **pos_args, **{k: v for k, v in loop_kw.items()})
@@ -739,9 +774,9 @@ def main():
         h2d = states[0].bytes_h2d()
         d2h = host_ids.numel() * 8
 
-        # ---- roofline pass (rank 0): one sample with every launch bracketed by CUDA events
+        # ---- roofline pass (--profile; rank 0): one more sample with every launch bracketed by CUDA events
         prof = None
-        if rank == 0 or tp_mode:  # tensor-parallel: every rank must take part (the forward contains collectives)
+        if args.profile and (rank == 0 or tp_mode):  # tensor-parallel: every rank must take part (the forward contains collectives)
             _lib.lib.mmdp_prof_enable(1)
             denoise_loop(new_state(), generator=rng, **loop_kw)
             prof = _lib.prof_summary()
@@ -751,7 +786,7 @@ def main():
     # ---- sub-records on the other BASELINE configs (every rank takes part where a collective or a barrier is involved)
     extras = {}
     states = st = None  # (they hold the model and ~120 MB of device buffers each)
-    if not tp_mode and not args.no_extras:
+    if not tp_mode and args.extras:
         if world > 1:
             try:
                 extras["tp"] = measure_tensor_parallel(args, model_cfg, device, rank, world, model, steps=max(1, min(args.steps, 3)))
@@ -772,61 +807,61 @@ def main():
     n_samples = args.steps if tp_mode else world * args.steps
     total_tokens = n_samples * TOKENS_PER_SAMPLE
     value = total_tokens / (ms_value / 1e3)
-    e2e_value = total_tokens / (ms_e2e / 1e3)
+    e2e_tokens = (1 if tp_mode else world) * e2e_steps * TOKENS_PER_SAMPLE
+    e2e_value = e2e_tokens / (ms_e2e / 1e3) if e2e_steps else None
     peak_tf, peak_src, peaks = load_peaks()
-    gemm_ms, gemm_flops, gemm_n = prof["gemm"]
-    att_ms, att_flops, att_n = prof["attention"]
-    row_ms, row_bytes, row_n = prof["row"]
-    smp_ms, smp_bytes, smp_n = prof["sampling"]
-    achieved = gemm_flops / (gemm_ms / 1e3) / 1e12 if gemm_ms else 0.0
-    traffic = None
-    try:
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "roofline_traffic.json"))).get("gemm_dram_bytes_per_launch")
-    except Exception:
-        pass
     flops_sample = algorithmic_flops_per_sample(model_cfg)
-    hbm = peaks.get("hbm_gbs", 6650.0)
     out = {
         "metric": "denoised_tokens_per_sec", "value": value, "unit": "tokens/s", "n_gpus": world, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": ms_value / args.steps, "higher_is_better": True,
         "scaling": "strong" if tp_mode else "weak", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
         "config": workload_config(args, world),
         "e2e": {"value": e2e_value, "unit": "tokens/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
-                "ms_per_step": ms_e2e / args.steps},
+                "ms_per_step": ms_e2e / e2e_steps if e2e_steps else None, "steps": e2e_steps},
         "gpu_launches": launches,
         "clocks": clock_info,
-        "roofline": {"kernel": "gemm_pair_kernel / gemm_bf16_kernel (tcgen05 cta_group::2 / ::1, all epilogues)", "bound": "tensor", "achieved": achieved, "peak": peak_tf,
-                     "unit": "TFLOP/s", "frac": achieved / peak_tf if peak_tf else None, "traffic": traffic,
-                     "peak_source": peak_src, "launches": gemm_n, "avg_launch_ms": gemm_ms / max(1, gemm_n),
-                     "algorithmic_flops_per_launch": gemm_flops / max(1, gemm_n)},
-        "kernel_breakdown_one_sample_ms": {"gemm": gemm_ms, "attention": att_ms, "row_kernels": row_ms, "sampling": smp_ms,
-                                           "attention_tflops": att_flops / (att_ms / 1e3) / 1e12 if att_ms else None,
-                                           "row_GBps": row_bytes / (row_ms / 1e3) / 1e9 if row_ms else None,
-                                           "sampling_GBps": smp_bytes / (smp_ms / 1e3) / 1e9 if smp_ms else None,
-                                           "sampling_frac_of_hbm_peak": (smp_bytes / (smp_ms / 1e3) / 1e9 / hbm) if smp_ms else None,
-                                           "note": "per-launch CUDA events serialise the launches: programmatic dependent launch overlap is "
-                                                   "not visible here, the timed regions above include it"},
-        # executed tensor work of one sample = the flops of the GEMM and attention launches actually made (profiled sample). It is
-        # below BASELINE.md's "minimal-equivalent" 7.101 PFLOP: the last block computes its attention output / MLP only for the
-        # rows whose logits are read (row window, output-invariant), 0.11 PFLOP per sample less.
-        "executed_pflop_per_sample": (gemm_flops + att_flops) / 1e15,
         "baseline_minimal_pflop_per_sample": flops_sample / 1e15,
-        "whole_step_tflops_executed_work": (gemm_flops + att_flops) * n_samples / (ms_value / 1e3) / 1e12,
-        "whole_step_frac_of_peak": (gemm_flops + att_flops) * n_samples / (ms_value / 1e3) / 1e12 / (peak_tf * world),  # per-GPU fraction
+        "roofline": None, "kernel_breakdown_one_sample_ms": None,
     }
+    if prof is not None:
+        gemm_ms, gemm_flops, gemm_n = prof["gemm"]
+        att_ms, att_flops, att_n = prof["attention"]
+        row_ms, row_bytes, row_n = prof["row"]
+        smp_ms, smp_bytes, smp_n = prof["sampling"]
+        achieved = gemm_flops / (gemm_ms / 1e3) / 1e12 if gemm_ms else 0.0
+        hbm = peaks.get("hbm_gbs", 3350.0)  # H100 SXM data sheet
+        out.update({
+            "roofline": {"kernel": "gemm_bf16_kernel (wgmma, all epilogues)", "bound": "tensor", "achieved": achieved, "peak": peak_tf,
+                         "unit": "TFLOP/s", "frac": achieved / peak_tf if peak_tf else None,
+                         "peak_source": peak_src, "launches": gemm_n, "avg_launch_ms": gemm_ms / max(1, gemm_n),
+                         "algorithmic_flops_per_launch": gemm_flops / max(1, gemm_n)},
+            "kernel_breakdown_one_sample_ms": {"gemm": gemm_ms, "attention": att_ms, "row_kernels": row_ms, "sampling": smp_ms,
+                                               "attention_tflops": att_flops / (att_ms / 1e3) / 1e12 if att_ms else None,
+                                               "row_GBps": row_bytes / (row_ms / 1e3) / 1e9 if row_ms else None,
+                                               "sampling_GBps": smp_bytes / (smp_ms / 1e3) / 1e9 if smp_ms else None,
+                                               "sampling_frac_of_hbm_peak": (smp_bytes / (smp_ms / 1e3) / 1e9 / hbm) if smp_ms else None,
+                                               "note": "per-launch CUDA events serialise the launches: programmatic dependent launch overlap is "
+                                                       "not visible here, the timed regions above include it"},
+            # executed tensor work of one sample = the flops of the GEMM and attention launches actually made (profiled sample). It is
+            # below BASELINE.md's "minimal-equivalent" 7.101 PFLOP: the last block computes its attention output / MLP only for the
+            # rows whose logits are read (row window, output-invariant), 0.11 PFLOP per sample less.
+            "executed_pflop_per_sample": (gemm_flops + att_flops) / 1e15,
+            "whole_step_tflops_executed_work": (gemm_flops + att_flops) * n_samples / (ms_value / 1e3) / 1e12,
+            "whole_step_frac_of_peak": (gemm_flops + att_flops) * n_samples / (ms_value / 1e3) / 1e12 / (peak_tf * world),  # per-GPU fraction
+        })
     out.update(extras)
     if world == 1 and not tp_mode:
-        if not args.no_cpu_baseline:
+        if args.cpu_baseline:
             r = cpu_reference_sample(model_cfg)
             out["cpu_baseline"] = {"value": r["tokens_per_s"], "unit": "tokens/s", "cores": r["cores"], "kind": "port",
                                    "sample": r["sample"], "sec_per_sample": r["sec_per_sample"], "cpu": r["cpu"],
                                    "thread_sweep_sec_per_block": r["thread_sweep_sec_per_block"]}
         else:
             out["cpu_baseline"] = None
-        if not args.no_extras:
+        if args.extras:
             try:
                 g = gpu_eager_baseline(model_cfg, device, lay)
-                g["speedup_e2e_over_eager"] = e2e_value / g["value"]
+                g["speedup_e2e_over_eager"] = e2e_value / g["value"] if e2e_value else None
                 out["gpu_eager_baseline"] = g
             except Exception as e:
                 out["gpu_eager_baseline"] = {"error": f"{type(e).__name__}: {e}"[:400]}

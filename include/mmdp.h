@@ -1,5 +1,5 @@
 /*
- * mmdp.h - C ABI of the B200-native MMaDA-Parallel denoising hot path (libmmdp.so).
+ * mmdp.h - C ABI of the H100-native (sm_90a) MMaDA-Parallel denoising hot path (libmmdp.so).
  *
  * The reference (tyfeld/MMaDA-Parallel) has no FFI/plugin layer: its boundary is the Python API
  *   generate_ti2ti(...)                         MMaDA-Parallel-A/generators/parallel_generator.py:102-368
@@ -41,9 +41,9 @@ MMDP_API const char* mmdp_last_error(void);
 MMDP_API void mmdp_prof_enable(int on);
 MMDP_API int mmdp_prof_summary(double* ms, double* work, long long* launches);
 MMDP_API long long mmdp_launch_count(int reset);
-/* Kernel selection for GEMMs with M > 256: 1 (default) = CTA pair per 256xN tile (cta_group::2), 0 = one CTA per 128xN tile
- * (cta_group::1, with its split-K tail), 2 = pair kernel only for M >= 4096 and N >= 8192. Without the split-K tail the two
- * kernels are bit-identical (same K order); also settable with the environment variable MMDP_GEMM_PAIR. */
+/* Kernel selection for GEMMs: 0 (default) = one CTA per 128xN tile (with its split-K tail), 1 = for M > 256 a cluster of two
+ * CTAs per pair of m-adjacent 128xN tiles, the W tile multicast to both (TMA multicast), 2 = pairs only for M >= 4096 and
+ * N >= 8192. Without the split-K tail the two kernels are bit-identical (same K order); also MMDP_GEMM_PAIR. */
 MMDP_API void mmdp_set_gemm_pair(int on);
 /* Split-K tail of the persistent GEMM (csrc/gemm.cu): 0 = never, 1 = residual epilogues only, 2 (default) = every epilogue
  * where the launch planner's cost model says it pays, 3 = whenever a partial last wave exists (tests).
@@ -53,12 +53,12 @@ MMDP_API void mmdp_set_gemm_pair(int on);
  * cooperative (co-residency of the grid is guaranteed by the runtime). Also MMDP_GEMM_SPLITK. */
 MMDP_API void mmdp_set_gemm_splitk(int mode);
 /* Programmatic dependent launch between the kernels of a forward (1 = default): a kernel's prologue (barrier init,
- * tensor-memory allocation, descriptor prefetch) overlaps the tail of its predecessor; every kernel waits for the
+ * descriptor prefetch) overlaps the tail of its predecessor; every kernel waits for the
  * predecessor's completion (griddepcontrol.wait) before touching its data. Also MMDP_PDL=0|1. */
 MMDP_API void mmdp_set_pdl(int on);
 /* Generic tuning knob (bench/profiling tools): keys "pdl", "gemm_splitk", "gemm_l2pf" (L2 prefetch distance of weight tiles
- * in k-blocks, 0 = off), "gemm_l2pf_mod", "gemm_pair", "gemm_group_m", "attn_split_tail" (KV-split of attention's partial
- * last wave), "attn_poly", "rmsnorm_warp". Each defaults to the environment variable MMDP_<KEY in upper case>. */
+ * in k-blocks, 0 = off), "gemm_l2pf_mod", "gemm_pair", "gemm_group_m", "attn_split_tail" (KV-split of attention's
+ * partial last wave), "attn_version" (6: 128-key blocks, 7: 64-key blocks), "rmsnorm_warp", "row_window". Each defaults to the environment variable MMDP_<KEY in upper case>. */
 MMDP_API int mmdp_set_option(const char* key, int value);
 
 /* ---- tensor-parallel collective over NVLink peer memory (BASELINE config 4; csrc/tp_collective.cu) --------------------------
@@ -137,7 +137,7 @@ MMDP_API int mmdp_tp_forward(const mmdp_tp_ctx* c, const int64_t* ids, int B, in
 #define MMDP_EPI_F32 4     /* C (float*) = raw fp32 accumulators: tensor-parallel partial sums, all-reduced before rounding      */
 #define MMDP_EPI_SWIGLU 3  /* C = bf16(bf16(silu(bf16 g)) * bf16 u), W rows interleaved 128 gate / 128 up   :962-967 */
 
-/* C[M,N] = A[M,K] * W[N,K]^T, bf16 in, fp32 accumulate (tcgen05/TMEM), fused epilogue.
+/* C[M,N] = A[M,K] * W[N,K]^T, bf16 in, fp32 accumulate (wgmma), fused epilogue.
  * lda/ldw/ldc/ldr are row strides in elements (multiples of 8). For MMDP_EPI_SWIGLU, C has N/2 columns. */
 MMDP_API int mmdp_gemm_bf16(int epilogue, const uint16_t* A, int lda, const uint16_t* W, int ldw, int M, int N, int K,
                    uint16_t* C, int ldc, const uint16_t* R, int ldr, void* stream);

@@ -1,4 +1,4 @@
-"""mmada_parallel_b200 - B200-native (sm_100a) implementation of the MMaDA-Parallel parallel-denoising hot path.
+"""mmada_parallel_b200 - H100-native (sm_90a) implementation of the MMaDA-Parallel parallel-denoising hot path.
 
 Public surface mirrors the reference's inference API for that path only:
   mmada_parallel_b200.model.LLaDAForMultiModalGeneration        (A/model/modeling_xllmx_dimoo.py)

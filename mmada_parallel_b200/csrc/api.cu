@@ -317,8 +317,8 @@ MMDP_API int mmdp_tp_forward(const mmdp_tp_ctx* c, const int64_t* ids, int B, in
 
 MMDP_API void mmdp_prof_enable(int on) { prof_enable(on); }
 MMDP_API int mmdp_prof_summary(double* ms, double* work, long long* launches) { return prof_summary(ms, work, launches); }
-MMDP_API long long mmdp_launch_count(int reset) { return launch_count(reset); }
 MMDP_API void mmdp_set_gemm_pair(int on) { set_gemm_pair_mode(on); }
+MMDP_API long long mmdp_launch_count(int reset) { return launch_count(reset); }
 MMDP_API void mmdp_set_gemm_splitk(int mode) { set_gemm_splitk_mode(mode < 0 ? 0 : (mode > 3 ? 3 : mode)); }
 MMDP_API void mmdp_set_pdl(int on) { set_pdl_mode(on); }
 MMDP_API int mmdp_set_option(const char* key, int value) { return key ? set_opt(key, value) : set_error("mmdp_set_option: null key"); }

@@ -1,4 +1,4 @@
-// TF32 tcgen05 "shifted-tap" GEMM: the convolution engine of the VQ decoders (MAGVITv2.decode_code,
+// TF32 wgmma "shifted-tap" GEMM: the convolution engine of the VQ decoders (MAGVITv2.decode_code,
 // MMaDA-Parallel-M/models/modeling_magvitv2.py:365-399,429-433; blocks in models/common_modules.py).
 //
 //   C[m, n] = bias + sum_{t < T} sum_k A[m + shift[t], k] * W[t*N + n, k]   (+ R[m, n])          fp32 in / fp32 out
@@ -6,9 +6,9 @@
 // Activations are channels-last fp32 with a one-pixel zero border per image ("padded NHWC": row index
 // (y+1)*(W+2) + (x+1), C contiguous), so a 3x3 convolution is nine GEMM taps whose A tiles are the SAME activation
 // matrix read at nine row offsets - a TMA tile load with a shifted row coordinate (out-of-range rows read as zero).
-// All taps accumulate into one TMEM accumulator (K loop = taps x channel blocks); kind::tf32 MMAs consume the fp32
+// All taps accumulate into one register accumulator (K loop = taps x channel blocks); tf32 wgmma consumes the fp32
 // tiles directly (10-bit mantissa, what cuDNN does for the reference on a GPU with allow_tf32). 1x1 convolutions and
-// the AttnBlock matmuls are the T = 1 case. Same warp-specialised pipeline as gemm.cu (TMA / MMA / epilogue warps).
+// the AttnBlock matmuls are the T = 1 case. Same warp-specialised pipeline as gemm.cu (TMA warpgroup, two MMA warpgroups).
 #include "mmdp_internal.h"
 #include "ptx.cuh"
 
@@ -19,7 +19,7 @@ static constexpr int kCStages = 6;
 static constexpr int kCABytes = CBM * CBK * 4;  // 16 KB
 static constexpr int kCBBytes = CBN * CBK * 4;  // 16 KB
 static constexpr int kCStageBytes = kCABytes + kCBBytes;
-static constexpr int kConvThreads = 256;
+static constexpr int kConvThreads = 384;
 static constexpr int kConvSmem = kCStages * kCStageBytes + 1024 + 256;
 static constexpr int kMaxTaps = 9;
 
@@ -40,51 +40,30 @@ struct ConvParams {
     int scatter_h;
 };
 
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(uint32_t M, uint32_t N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_tf32_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc)
-        : "memory");
-}
-
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const ConvParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kCStages * kCStageBytes);
     uint64_t* empty_bar = full_bar + kCStages;
-    uint64_t* tmem_full = empty_bar + kCStages;
-    uint64_t* tmem_empty = tmem_full + 2;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmW);
-    }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < kCStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(&tmem_full[s], 1); mbar_init(&tmem_empty[s], 4); }
+        for (int s = 0; s < kCStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
         fence_barrier_init();
     }
-    if (warp == 2) tmem_alloc<256>(tmem_ptr);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
     const int num_m = (p.M + CBM - 1) / CBM, num_n = (p.N + CBN - 1) / CBN;
     const int kblocks = p.K / CBK;
     const int num_k = p.T * kblocks;
     const int num_tiles = num_m * num_n;
 
-    if (warp == 0) {
-        if (elect_one_sync()) {
+    if (wg == 0) {
+        setmaxnreg_dec<40>();
+        if (warp == 0 && elect_one_sync()) {
             int s = 0; uint32_t ph = 0;
             for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
                 const int n_blk = tile % num_n, m_blk = tile / num_n;  // n fastest: CTAs running together share the A rows
@@ -100,88 +79,71 @@ conv_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
         }
         __syncwarp();
-    } else if (warp == 1) {
-        if (elect_one_sync()) {
-            constexpr uint32_t idesc = umma_idesc_tf32(CBM, CBN);
-            int s = 0; uint32_t ph = 0; int as = 0; uint32_t aph = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-                mbar_wait(&tmem_empty[as], aph ^ 1);
-                tcgen05_fence_after();
-                const uint32_t d_tmem = tmem_base + as * CBN;
-                for (int kb = 0; kb < num_k; ++kb) {
-                    mbar_wait(&full_bar[s], ph);
-                    tcgen05_fence_after();
-                    const uint32_t sa = smem_u32(smem + s * kCStageBytes);
-                    const uint64_t adesc = umma_desc_kmajor_sw128(sa), bdesc = umma_desc_kmajor_sw128(sa + kCABytes);
-#pragma unroll
-                    for (int k = 0; k < CBK / 8; ++k)  // UMMA_K = 8 for tf32: 32 bytes per step inside the swizzle atom
-                        umma_tf32_ss(d_tmem, adesc + k * 2, bdesc + k * 2, idesc, (kb | k) != 0);
-                    umma_commit(&empty_bar[s]);
-                    if (kb == num_k - 1) umma_commit(&tmem_full[as]);
-                    if (++s == kCStages) { s = 0; ph ^= 1; }
-                }
-                if (++as == 2) { as = 0; aph ^= 1; }
-            }
-        }
-        __syncwarp();
-    } else if (warp >= 4) {
-        const int ew = warp - 4;
-        int as = 0; uint32_t aph = 0;
+    } else {
+        setmaxnreg_inc<232>();
+        const int half = wg - 1;
+        const int rit0 = half * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+        float acc[CBN / 2];
+        int s = 0; uint32_t ph = 0;
         for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             const int n_blk = tile % num_n, m_blk = tile / num_n;
-            mbar_wait(&tmem_full[as], aph);
-            tcgen05_fence_after();
-            const int row = m_blk * CBM + ew * 32 + lane;
-            bool row_ok = row < p.M;
-            bool interior = true;
-            long long orow = row;
-            if (p.pad_w > 0 && row_ok) {
-                const int per = p.pad_w * p.pad_h;
-                const int r = row % per;
-                const int y = r / p.pad_w, x = r - y * p.pad_w;
-                interior = (y >= 1) && (y <= p.pad_h - 2) && (x >= 1) && (x <= p.pad_w - 2);
-            } else if (p.scatter_w > 0 && row_ok) {
-                const int per = p.scatter_w * p.scatter_h;
-                const int b = row / per, r = row - b * per;
-                const int y = r / p.scatter_w, x = r - y * p.scatter_w;
-                orow = (long long)b * (p.scatter_w + 2) * (p.scatter_h + 2) + (long long)(y + 1) * (p.scatter_w + 2) + (x + 1);
-            }
-            const uint32_t tbase = tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + as * CBN;
-#pragma unroll 1
-            for (int c = 0; c < CBN / 32; ++c) {
-                uint32_t v[32];
-                tmem_ld_32x32b_x32(tbase + c * 32, v);
-                tmem_ld_wait();
-                const int col0 = n_blk * CBN + c * 32;
-                if (row_ok && col0 < p.N) {
-                    float* dst = p.C + orow * p.ldc + col0;
-                    const float* rsd = p.R ? p.R + orow * p.ldr + col0 : nullptr;
-                    const float bm = (p.bias && p.bias_along_m) ? p.bias[row] : 0.f;
+            int prev_s = -1;
+            for (int kb = 0; kb < num_k; ++kb) {
+                mbar_wait(&full_bar[s], ph);
+                const uint32_t sa = smem_u32(smem + s * kCStageBytes);
+                const uint64_t adesc = smem_desc_kmajor_sw128(sa + half * (64 * 128)), bdesc = smem_desc_kmajor_sw128(sa + kCABytes);
+                wgmma_fence();
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        if (col0 + i < p.N) {
+                for (int k = 0; k < CBK / 8; ++k)  // K = 8 per tf32 wgmma: 32 bytes per step inside the swizzle atom
+                    wgmma_tf32_ss_n128(acc, adesc + k * 2, bdesc + k * 2, (kb | k) != 0);
+                wgmma_commit();
+                wgmma_wait<1>();
+                reg_fence(acc);
+                if (prev_s >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_s]);
+                prev_s = s;
+                if (++s == kCStages) { s = 0; ph ^= 1; }
+            }
+            wgmma_wait<0>();
+            reg_fence(acc);
+            if (prev_s >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_s]);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = m_blk * CBM + rit0 + 8 * h;
+                if (row >= p.M) continue;
+                bool interior = true;
+                long long orow = row;
+                if (p.pad_w > 0) {
+                    const int per = p.pad_w * p.pad_h;
+                    const int r = row % per;
+                    const int y = r / p.pad_w, x = r - y * p.pad_w;
+                    interior = (y >= 1) && (y <= p.pad_h - 2) && (x >= 1) && (x <= p.pad_w - 2);
+                } else if (p.scatter_w > 0) {
+                    const int per = p.scatter_w * p.scatter_h;
+                    const int b = row / per, r = row - b * per;
+                    const int y = r / p.scatter_w, x = r - y * p.scatter_w;
+                    orow = (long long)b * (p.scatter_w + 2) * (p.scatter_h + 2) + (long long)(y + 1) * (p.scatter_w + 2) + (x + 1);
+                }
+                float* dst = p.C + orow * p.ldc;
+                const float* rsd = p.R ? p.R + orow * p.ldr : nullptr;
+                const float bm = (p.bias && p.bias_along_m) ? p.bias[row] : 0.f;
+#pragma unroll
+                for (int j = 0; j < CBN / 8; ++j) {
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int col = n_blk * CBN + 8 * j + c0 + e;
+                        if (col < p.N) {
                             float o = 0.f;
                             if (interior) {
-                                o = __uint_as_float(v[i]) * p.alpha;
-                                if (p.bias) o += p.bias_along_m ? bm : p.bias[col0 + i];
-                                if (rsd) o += rsd[i];
+                                o = acc[4 * j + 2 * h + e] * p.alpha;
+                                if (p.bias) o += p.bias_along_m ? bm : p.bias[col];
+                                if (rsd) o += rsd[col];
                             }
-                            dst[i] = o;
+                            dst[col] = o;
                         }
                     }
                 }
             }
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[as]);
-            if (++as == 2) { as = 0; aph ^= 1; }
         }
-    }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tcgen05_fence_after();
-        tmem_dealloc<256>(tmem_base);
     }
 }
 
@@ -425,14 +387,14 @@ __global__ void lfq_indices_kernel(const float* __restrict__ z, int64_t* __restr
 
 int nchw_to_padded(const float* x, float* y, int B, int C, int Cpad, int H, int W, cudaStream_t stream) {
     LaunchScope ls(LK_ROW, (double)B * H * W * (C + Cpad) * 4, stream);
-    nchw_to_padded_kernel<<<dim3(148 * 4, B), 256, 0, stream>>>(x, y, C, Cpad, H, W);
+    nchw_to_padded_kernel<<<dim3(num_sms() * 4, B), 256, 0, stream>>>(x, y, C, Cpad, H, W);
     MMDP_CUDA(cudaGetLastError());
     return 0;
 }
 int downsample_pick(const float* src, float* dst, int B, int C, int H, int W, cudaStream_t stream) {
     if ((C % 4) || (H % 2) || (W % 2)) return set_error("downsample: C %% 4 and even H, W required");
     LaunchScope ls(LK_ROW, (double)B * (H / 2) * (W / 2) * C * 8, stream);
-    downsample_pick_kernel<<<dim3(148 * 4, B), 256, 0, stream>>>(src, dst, C, H, W);
+    downsample_pick_kernel<<<dim3(num_sms() * 4, B), 256, 0, stream>>>(src, dst, C, H, W);
     MMDP_CUDA(cudaGetLastError());
     return 0;
 }
@@ -449,7 +411,7 @@ int gn_swish(const float* x, float* y, int B, int C, int H, int W, double* stats
     MMDP_CUDA(cudaMemsetAsync(stats_ws, 0, (size_t)B * 32 * 2 * sizeof(double), stream));
     const long long npix = (long long)H * W;
     int chunks = (int)((npix + 127) / 128);
-    if (chunks > 148 * 16) chunks = 148 * 16;
+    if (chunks > num_sms() * 16) chunks = num_sms() * 16;
     {
         LaunchScope ls(LK_ROW, (double)B * npix * C * 4, stream);
         gn_stats_kernel<<<dim3(chunks, B), 256, 0, stream>>>(x, C, H, W, stats_ws);
@@ -464,7 +426,7 @@ int gn_swish(const float* x, float* y, int B, int C, int H, int W, double* stats
 int upsample2x(const float* x, float* y, int B, int C, int H, int W, cudaStream_t stream) {
     if (C % 4) return set_error("upsample: channels must be a multiple of 4");
     LaunchScope ls(LK_ROW, (double)B * H * W * C * 4 * 5, stream);
-    upsample2x_kernel<<<dim3(148 * 8, B), 256, 0, stream>>>(x, y, C, H, W);
+    upsample2x_kernel<<<dim3(num_sms() * 8, B), 256, 0, stream>>>(x, y, C, H, W);
     MMDP_CUDA(cudaGetLastError());
     return 0;
 }
@@ -507,7 +469,7 @@ int lfq_to_padded(const int64_t* ids, float* z, int B, int H, int W, int bits, i
 
 int padded_to_nchw(const float* x, float* y, int B, int C, int ld, int H, int W, cudaStream_t stream) {
     LaunchScope ls(LK_ROW, (double)B * C * H * W * 8, stream);
-    padded_to_nchw_kernel<<<dim3(148 * 4, B), 256, 0, stream>>>(x, y, C, ld, H, W);
+    padded_to_nchw_kernel<<<dim3(num_sms() * 4, B), 256, 0, stream>>>(x, y, C, ld, H, W);
     MMDP_CUDA(cudaGetLastError());
     return 0;
 }

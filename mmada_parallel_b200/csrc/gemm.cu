@@ -1,9 +1,8 @@
-// Persistent warp-specialised bf16 GEMM for sm_100a:  C[M,N] = A[M,K] · W[N,K]^T  (fp32 accumulate in TMEM)
+// Persistent warp-specialised bf16 GEMM for sm_90a:  C[M,N] = A[M,K] · W[N,K]^T  (fp32 accumulate in registers)
 //
-//   warp 0      : TMA producer   (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx)
-//   warp 1      : MMA issuer     (one thread issues tcgen05.mma 128x256x16, tcgen05.commit frees smem slots)
-//   warp 2      : TMEM allocator (512 columns = 2 accumulator stages of 128x256 fp32)
-//   warps 4..7  : epilogue       (tcgen05.ld 32x32b, fused epilogue, global stores) - overlaps the next tile's MMAs
+//   warpgroup 0    : TMA producer  (one elected thread: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx)
+//   warpgroups 1,2 : MMA + epilogue (wgmma m64nBNk16, one 64-row half of the 128 x BN tile each; the fused epilogue runs
+//                    on the register fragments while the producer already fills the ring with the next tile's k-blocks)
 //
 // Every nn.Linear of the reference block (MMaDA-Parallel-A/model/modeling_llada.py:925-927, :744, :962, :968, :1402)
 // maps to one launch of this kernel with a fused epilogue that reproduces the reference's bf16 rounding points:
@@ -23,16 +22,15 @@ namespace mmdp {
 
 static constexpr int BM = 128, BK = 64;
 static constexpr int kABytes = BM * BK * 2;  // 16 KB
-static constexpr int kGemmThreads = 256;
+static constexpr int kGemmThreads = 384;
 // The N tile width is a template parameter: 256 (default; required by the QKV/SwiGLU epilogues) or 192. The K loop and
 // therefore the fp32 accumulation order of every output element is identical for both, so results do not depend on
-// the tile width; the host picks the width that minimises (waves x width) for the problem (wave quantisation on 148 SMs).
+// the tile width; the host picks the width that minimises (waves x width) for the problem (wave quantisation on the SMs).
 template <int BN> struct GemmCfg {
     static constexpr int kBBytes = BN * BK * 2;
     static constexpr int kStageBytes = kABytes + kBBytes;
-    static constexpr int kStages = (BN == 256) ? 4 : 5;
-    static constexpr int kScatBytes = 4 * kScatStageFloats * 4;  // staging of the fused reduce-scatter epilogue (EPI_F32)
-    static constexpr int kSmem = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/ + kScatBytes;
+    static constexpr int kStages = (BN == 256) ? 4 : 5;  // 192 / 200 KB of the 227 KB an H100 block may use
+    static constexpr int kSmem = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
 template <int EPI, int BN>
@@ -45,34 +43,21 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
     uint64_t* empty_bar = full_bar + kStages;
-    uint64_t* tmem_full = empty_bar + kStages;
-    uint64_t* tmem_empty = tmem_full + 2;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-    float* scat_stage = reinterpret_cast<float*>(smem + kStages * kStageBytes + 256);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
+    const int wg = warp >> 2;
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
-    }
-    if (warp == 1 && lane == 0) {
         for (int s = 0; s < kStages; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(&tmem_full[s], 1);
-            mbar_init(&tmem_empty[s], 4);  // one arrive per epilogue warp
+            mbar_init(&empty_bar[s], 8);  // one arrive per MMA warp
         }
         fence_barrier_init();
     }
-    if (warp == 2) tmem_alloc<512>(tmem_ptr);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
     // everything above overlaps the tail of the previous kernel in the stream (programmatic dependent launch)
     pdl_launch_dependents();
     pdl_wait();
@@ -91,9 +76,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const int unit_kb0 = unit_s * p.sk_kb_per;
     const int unit_kb1 = (unit_kb0 + p.sk_kb_per < num_k) ? unit_kb0 + p.sk_kb_per : num_k;
 
-    if (warp == 0) {
+    if (wg == 0) {
         // ===================== TMA producer =====================
-        if (elect_one_sync()) {
+        setmaxnreg_dec<40>();
+        if (warp == 0 && elect_one_sync()) {
             int s = 0;
             uint32_t ph = 0;
             for (int tile = blockIdx.x; tile < full_tiles + (has_unit ? 1 : 0) * gridDim.x; tile += gridDim.x) {
@@ -118,104 +104,188 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
         }
         __syncwarp();
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        if (elect_one_sync()) {
-            constexpr uint32_t idesc = umma_idesc_bf16(BM, BN);
-            int s = 0;
-            uint32_t ph = 0;
-            int as = 0;
-            uint32_t aph = 0;
-            for (int tile = blockIdx.x; tile < full_tiles + (has_unit ? 1 : 0) * gridDim.x; tile += gridDim.x) {
-                const bool is_unit = tile >= full_tiles;
-                const int kb_beg = is_unit ? unit_kb0 : 0, kb_end = is_unit ? unit_kb1 : num_k;
-                mbar_wait(&tmem_empty[as], aph ^ 1);
-                tcgen05_fence_after();
-                const uint32_t d_tmem = tmem_base + as * BN;
-                for (int kb = kb_beg; kb < kb_end; ++kb) {
-                    mbar_wait(&full_bar[s], ph);
-                    tcgen05_fence_after();
-                    const uint32_t sa = smem_u32(smem + s * kStageBytes);
-                    const uint64_t adesc = umma_desc_kmajor_sw128(sa);
-                    const uint64_t bdesc = umma_desc_kmajor_sw128(sa + kABytes);
-#pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {
-                        // +32 bytes per 16 bf16 of K inside the 128-B swizzle atom
-                        umma_bf16_ss(d_tmem, adesc + (k * 2), bdesc + (k * 2), idesc, ((kb - kb_beg) | k) != 0);
-                    }
-                    umma_commit(&empty_bar[s]);
-                    if (kb == kb_end - 1) umma_commit(&tmem_full[as]);
-                    if (++s == kStages) { s = 0; ph ^= 1; }
-                }
-                if (++as == 2) { as = 0; aph ^= 1; }
-                if (is_unit) break;
-            }
-        }
-        __syncwarp();
-    } else if (warp >= 4) {
-        // ===================== epilogue =====================
-        const int ew = warp - 4;  // == warp % 4 -> TMEM lane quarter
-        int as = 0;
-        uint32_t aph = 0;
+    } else {
+        // ===================== MMA + epilogue (warpgroups 1 and 2: tile rows [64 (wg-1), 64 wg)) =====================
+        setmaxnreg_inc<232>();
+        const int half = wg - 1;
+        const int rit0 = half * 64 + (warp & 3) * 16 + (lane >> 2);  // tile row of acc[4j + 0..1]; acc[4j + 2..3] is 8 rows below
+        const int c0 = 2 * (lane & 3);
+        float acc[BN / 2];
+        int s = 0;
+        uint32_t ph = 0;
         for (int tile = blockIdx.x; tile < full_tiles + (has_unit ? 1 : 0) * gridDim.x; tile += gridDim.x) {
             const bool is_unit = tile >= full_tiles;
             const int tl = is_unit ? unit_tile : tile;
             int m_blk, n_blk;
             gemm_tile_coords(tl, num_m, num_n, p.group_m, m_blk, n_blk);
-            mbar_wait(&tmem_full[as], aph);
-            tcgen05_fence_after();
-            const int row = m_blk * BM + ew * 32 + lane;
-            const bool row_ok = row < p.M;
-            const uint32_t tbase = tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + as * BN;
-            bool run_epilogue = true;
+            const int kb_beg = is_unit ? unit_kb0 : 0, kb_end = is_unit ? unit_kb1 : num_k;
+            int prev_s = -1;
+            for (int kb = kb_beg; kb < kb_end; ++kb) {
+                mbar_wait(&full_bar[s], ph);
+                const uint32_t sa = smem_u32(smem + s * kStageBytes);
+                const uint64_t adesc = smem_desc_kmajor_sw128(sa + half * (64 * 128));
+                const uint64_t bdesc = smem_desc_kmajor_sw128(sa + kABytes);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k) {
+                    // +32 bytes per 16 bf16 of K inside the 128-B swizzle atom
+                    const int acc_in = ((kb - kb_beg) | k) != 0;
+                    if constexpr (BN == 256) wgmma_bf16_ss_n256(acc, adesc + k * 2, bdesc + k * 2, acc_in);
+                    else wgmma_bf16_ss_n192(acc, adesc + k * 2, bdesc + k * 2, acc_in);
+                }
+                wgmma_commit();
+                // keep this k-block's MMAs in flight; the previous k-block's have retired -> its stage goes back to the producer
+                wgmma_wait<1>();
+                reg_fence(acc);
+                if (prev_s >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_s]);
+                prev_s = s;
+                if (++s == kStages) { s = 0; ph ^= 1; }
+            }
+            wgmma_wait<0>();
+            reg_fence(acc);
+            if (prev_s >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_s]);
             if (is_unit) {
-                run_epilogue = false;
                 const int S = p.sk_splits;
-                const int rit = ew * 32 + lane;  // row in tile == TMEM lane of this thread
-                float4* tile_ws = reinterpret_cast<float4*>(p.sk_ws) + (size_t)unit_t * S * (BN / 4) * BM;
+                const int tid = threadIdx.x - 128;  // 0..255 over the two MMA warpgroups
+                float* tile_ws = p.sk_ws + (size_t)unit_t * S * (BN / 4) * BM * 4;
                 // (1) publish this unit's partial accumulator
-                sk_publish<BN>(tile_ws + (size_t)unit_s * (BN / 4) * BM, tbase, rit);
+                sk_publish<BN>(tile_ws + (size_t)unit_s * (BN / 4) * BM * 4, acc, rit0, c0);
                 __threadfence();
-                asm volatile("bar.sync 2, 128;" ::: "memory");  // the 4 epilogue warps
+                asm volatile("bar.sync 2, 256;" ::: "memory");  // the 8 MMA warps
                 // (2) wait until every unit of this tile has published. All units are co-resident: the launch is cooperative
                 //     (grid <= SMs x 1 CTA/SM is checked by the runtime), so a unit can only wait for CTAs that are running.
-                if (rit == 0) {
+                if (tid == 0) {
                     atomicAdd(p.sk_cnt + 2 * unit_t, 1);
                     uint32_t spins = 0;
                     while (*reinterpret_cast<volatile int*>(p.sk_cnt + 2 * unit_t) < S) {
-                        if (++spins > (1u << 26)) { printf("mmdp: split-K wait timeout tile %d\n", unit_t); __trap(); }
+                        if (++spins > (1u << 26)) __trap();
                     }
                     __threadfence();
                 }
-                asm volatile("bar.sync 2, 128;" ::: "memory");
+                asm volatile("bar.sync 2, 256;" ::: "memory");
                 // (3) distributed reduction + fused epilogue on the rows this unit owns (gemm_epilogue.cuh)
-                sk_finish<EPI, BN>(p, tile_ws, S, unit_s, m_blk, n_blk, rit);
+                sk_finish<EPI, BN>(p, reinterpret_cast<const float4*>(tile_ws), S, unit_s, m_blk, n_blk, tid);
                 // (4) the last unit to finish re-arms the counters for the next launch
-                asm volatile("bar.sync 2, 128;" ::: "memory");
-                if (rit == 0) {
+                asm volatile("bar.sync 2, 256;" ::: "memory");
+                if (tid == 0) {
                     const int old = atomicAdd(p.sk_cnt + 2 * unit_t + 1, 1);
                     if (old == S - 1) { p.sk_cnt[2 * unit_t] = 0; p.sk_cnt[2 * unit_t + 1] = 0; }
                 }
+                break;
             }
-            if (run_epilogue) gemm_epilogue_tile<EPI, BN>(p, tbase, row, row_ok, n_blk, scat_stage + ew * kScatStageFloats);
-            // all TMEM reads of this accumulator stage are complete (wait::ld above) -> hand it back to the MMA warp
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[as]);
-            if (++as == 2) { as = 0; aph ^= 1; }
-            if (is_unit) break;
+            gemm_epilogue_tile<EPI, BN>(p, acc, m_blk, n_blk, rit0, c0);
         }
         if constexpr (EPI == EPI_F32) {
             if (p.scat_R > 0) __threadfence_system();  // the pushed rows are visible to their owners before this grid completes
         }
     }
+}
 
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tcgen05_fence_after();
-        tmem_dealloc<512>(tmem_base);
+// CTA-pair variant (opt-in, MMDP_GEMM_PAIR=1): a cluster of two CTAs computes two m-adjacent 128 x BN tiles of the same n-tile.
+// Each CTA loads its own A tile and HALF of the shared W tile, multicast into both CTAs' shared memory, so a pair reads the
+// weights once per two m-tiles. A stage is refilled only when the MMA warps of BOTH CTAs have released it (their arrivals
+// go to both CTAs' empty barriers). The K loop of every output element is that of gemm_bf16_kernel without a split-K tail:
+// the results are bit-identical to it. On one H100 (700 W) the 8B benchmark ran at 70 tokens/s with pairs against 100 with
+// the 1-CTA kernel (GEMM time of a sample 16.9 s against 11.0 s), so the 1-CTA kernel is the default.
+template <int EPI, int BN>
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kGemmThreads, 1)
+gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBh, const GemmParams p) {
+    constexpr int kStages = GemmCfg<BN>::kStages;
+    constexpr int kStageBytes = GemmCfg<BN>::kStageBytes;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
+    uint64_t* empty_bar = full_bar + kStages;
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int wg = warp >> 2;
+    const uint32_t rank = cluster_ctarank();
+
+    if (warp == 0 && lane == 0) {
+        tma_prefetch_desc(&tmA);
+        tma_prefetch_desc(&tmBh);
+        for (int s = 0; s < kStages; ++s) {
+            mbar_init(&full_bar[s], 1);
+            mbar_init(&empty_bar[s], 16);  // one arrive per MMA warp of both CTAs
+        }
+        fence_barrier_init();
     }
+    cluster_sync();  // the peer's barriers are initialised before any multicast or remote arrive reaches them
+    pdl_launch_dependents();
+    pdl_wait();
+
+    const int num_m = (p.M + BM - 1) / BM;
+    const int num_n = (p.N + BN - 1) / BN;
+    const int num_k = (p.K + BK - 1) / BK;
+    const int num_pm = (num_m + 1) / 2;
+    const int pair_tiles = num_pm * num_n;
+    const int cid = blockIdx.x / 2, n_clusters = gridDim.x / 2;
+
+    if (wg == 0) {
+        // ===================== TMA producer =====================
+        setmaxnreg_dec<40>();
+        if (warp == 0 && elect_one_sync()) {
+            int s = 0;
+            uint32_t ph = 0;
+            for (int t = cid; t < pair_tiles; t += n_clusters) {
+                int pm, n_blk;
+                gemm_tile_coords(t, num_pm, num_n, p.group_m, pm, n_blk);
+                const int m_blk = 2 * pm + (int)rank;  // may be num_m for an odd count: rows read as zero, nothing is stored
+                for (int kb = 0; kb < num_k; ++kb) {
+                    mbar_wait(&empty_bar[s], ph ^ 1);
+                    mbar_expect_tx(&full_bar[s], kStageBytes);
+                    uint8_t* sa = smem + s * kStageBytes;
+                    tma_load_2d(sa, &tmA, &full_bar[s], kb * BK, m_blk * BM);
+                    tma_load_2d_multicast(sa + kABytes + rank * (BN / 2) * 128, &tmBh, &full_bar[s], kb * BK,
+                                          n_blk * BN + (int)rank * (BN / 2), 0x3);
+                    if (++s == kStages) { s = 0; ph ^= 1; }
+                }
+            }
+        }
+        __syncwarp();
+    } else {
+        // ===================== MMA + epilogue =====================
+        setmaxnreg_inc<232>();
+        const int half = wg - 1;
+        const int rit0 = half * 64 + (warp & 3) * 16 + (lane >> 2);
+        const int c0 = 2 * (lane & 3);
+        float acc[BN / 2];
+        int s = 0;
+        uint32_t ph = 0;
+        for (int t = cid; t < pair_tiles; t += n_clusters) {
+            int pm, n_blk;
+            gemm_tile_coords(t, num_pm, num_n, p.group_m, pm, n_blk);
+            const int m_blk = 2 * pm + (int)rank;
+            int prev_s = -1;
+            for (int kb = 0; kb < num_k; ++kb) {
+                mbar_wait(&full_bar[s], ph);
+                const uint32_t sa = smem_u32(smem + s * kStageBytes);
+                const uint64_t adesc = smem_desc_kmajor_sw128(sa + half * (64 * 128));
+                const uint64_t bdesc = smem_desc_kmajor_sw128(sa + kABytes);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k) {
+                    if constexpr (BN == 256) wgmma_bf16_ss_n256(acc, adesc + k * 2, bdesc + k * 2, (kb | k) != 0);
+                    else wgmma_bf16_ss_n192(acc, adesc + k * 2, bdesc + k * 2, (kb | k) != 0);
+                }
+                wgmma_commit();
+                wgmma_wait<1>();
+                reg_fence(acc);
+                if (prev_s >= 0 && lane == 0) { mbar_arrive(&empty_bar[prev_s]); mbar_arrive_cluster(&empty_bar[prev_s], rank ^ 1u); }
+                prev_s = s;
+                if (++s == kStages) { s = 0; ph ^= 1; }
+            }
+            wgmma_wait<0>();
+            reg_fence(acc);
+            if (prev_s >= 0 && lane == 0) { mbar_arrive(&empty_bar[prev_s]); mbar_arrive_cluster(&empty_bar[prev_s], rank ^ 1u); }
+            gemm_epilogue_tile<EPI, BN>(p, acc, m_blk, n_blk, rit0, c0);
+        }
+        if constexpr (EPI == EPI_F32) {
+            if (p.scat_R > 0) __threadfence_system();
+        }
+    }
+    cluster_sync();  // neither CTA exits while the other may still multicast into it or arrive on its barriers
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -299,7 +369,7 @@ static GemmPlan plan_gemm(int epi, int M, int N, int K) {
 }
 
 // Split-K workspace: one per (device, stream) - two streams running split GEMMs at the same time must not share partial
-// sums or arrival counters. 148 units x 128 KB + counters, allocated on first use, kept for the life of the process.
+// sums or arrival counters. 256 units (>= SMs) x 128 KB + counters, allocated on first use, kept for the life of the process.
 struct SkWorkspace { float* ws; int* cnt; };
 static std::map<std::pair<int, cudaStream_t>, SkWorkspace> g_sk;
 static std::mutex g_sk_mu;
@@ -317,6 +387,34 @@ static int splitk_workspace(cudaStream_t stream, SkWorkspace* out) {
     MMDP_CUDA(cudaMemsetAsync(w.cnt, 0, 2 * units * sizeof(int), stream));
     g_sk.emplace(key, w);
     *out = w;
+    return 0;
+}
+
+// CTA-pair launch: grid = 2 x the clusters that fit at once (1 CTA per SM; a GPC with an odd SM count leaves one SM out)
+template <int EPI, int BN>
+static int launch_gemm_pair(const CUtensorMap& tmA, const CUtensorMap& tmBh, const GemmParams& p, int pair_tiles, cudaStream_t stream) {
+    static int max_clusters[64] = {0};
+    int dev = 0;
+    MMDP_CUDA(cudaGetDevice(&dev));
+    int& mc = max_clusters[dev & 63];
+    if (mc == 0) {
+        MMDP_CUDA(cudaFuncSetAttribute(gemm_pair_kernel<EPI, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<BN>::kSmem));
+        cudaLaunchConfig_t cfg{};
+        cfg.gridDim = dim3(2 * num_sms());
+        cfg.blockDim = dim3(kGemmThreads);
+        cfg.dynamicSmemBytes = GemmCfg<BN>::kSmem;
+        cudaLaunchAttribute at{};
+        at.id = cudaLaunchAttributeClusterDimension;
+        at.val.clusterDim.x = 2; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
+        cfg.attrs = &at;
+        cfg.numAttrs = 1;
+        MMDP_CUDA(cudaOccupancyMaxActiveClusters(&mc, gemm_pair_kernel<EPI, BN>, &cfg));
+        if (mc < 1) return set_error("gemm_pair: no cluster of two CTAs fits on this device");
+    }
+    const int clusters = pair_tiles < mc ? pair_tiles : mc;
+    LaunchScope ls(LK_GEMM, 2.0 * p.M * (double)p.N * p.K, stream);
+    MMDP_CUDA(launch_ex(gemm_pair_kernel<EPI, BN>, dim3(2 * clusters), dim3(kGemmThreads), GemmCfg<BN>::kSmem, stream, pdl_mode() != 0,
+                        false, tmA, tmBh, p));
     return 0;
 }
 
@@ -356,13 +454,6 @@ int gemm_bf16(int epi, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, 
         default:
             return set_error("gemm: unknown epilogue");
     }
-    // kernel selection. Default (MMDP_GEMM_PAIR=1): problems with more than two m-tiles go to the CTA-pair (cta_group::2)
-    // kernel of gemm2.cu, whose 256 x BN tiles read a third less operand data per SM and flop - measured on the four body
-    // GEMMs of the bench workload (M = 2414): QKV +8.5 %, gate/up +5.7 %, attn_out +9 %, ff_out +1.6 %, one forward -3.8 %
-    // (profiles/r02). Small-M problems (the restricted LM head on 256 text rows) stay on the 1-CTA kernel below with its
-    // split-K tail. 0 = always 1-CTA, 2 = pair only for M >= 4096 and N >= 8192.
-    const int pm = gemm_pair_mode();
-    if ((pm == 1 && M > 256) || (pm == 2 && M >= 4096 && N >= 8192)) return gemm_bf16_pair(epi, A, lda, W, ldw, M, N, K, C, ldc, resid, ldr, qa, stream, sc);
     GemmParams p{};
     p.M = M; p.N = N; p.K = K;
     p.C = C; p.ldc = ldc; p.resid = resid; p.ldr = ldr;
@@ -379,11 +470,10 @@ int gemm_bf16(int epi, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, 
         p.scat_R = sc->rows_per_rank; p.scat_slot = sc->slot;
     }
     const int bn = pl.bn, grid = pl.grid;
-    // tile order (gemm_tile_coords): with many m-tiles, walk them in balanced groups of <= 40 so that one wave of 148 tiles
-    // spans ~30 m-tiles x ~5 n-tiles instead of all m-tiles x 2.6 n-tiles. Measured on M = 7242 (57 m-tiles, the B=3 batch
-    // of a caller that batches its CFG branches): +4..7 % on every body GEMM shape, DRAM reads 668 -> 362 MB; no gain below
-    // ~45 m-tiles, so M = 2414 keeps the plain order (profiles/r01/README.md). MMDP_GEMM_GROUP_M overrides: 0 = off, n > 0 =
-    // fixed group size.
+    // tile order (gemm_tile_coords): with many m-tiles, walk them in balanced groups of <= 40 so that one wave of tiles
+    // spans ~30 m-tiles x a few n-tiles instead of all m-tiles x 2-3 n-tiles, which keeps the wave's A rows in L2 while the
+    // weights stream (M = 7242: 57 m-tiles, the B=3 batch of a caller that batches its CFG branches); below ~45 m-tiles
+    // the plain order is kept (M = 2414). MMDP_GEMM_GROUP_M overrides: 0 = off, n > 0 = fixed group size.
     const int group_m_env = opt(OPT_GEMM_GROUP_M);
     {
         const int num_m = (M + BM - 1) / BM;
@@ -393,6 +483,29 @@ int gemm_bf16(int epi, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, 
             g = (num_m + ngroups - 1) / ngroups;
         }
         p.group_m = group_m_env >= 0 ? group_m_env : g;
+    }
+    if (qa) {
+        p.q = qa->q; p.k = qa->k; p.vt = qa->vt; p.cos_tab = qa->cos_tab; p.sin_tab = qa->sin_tab;
+        p.L = qa->L; p.Lpad = qa->Lpad; p.d_model = qa->d_model; p.n_heads = qa->n_heads;
+        p.pos_map = qa->pos_map; p.Tq = qa->Tq; p.row0 = qa->row0;
+    }
+    // kernel selection: MMDP_GEMM_PAIR / mmdp_set_gemm_pair 0 (default) = one CTA per tile (with the split-K tail), 1 = CTA
+    // pairs for M > 256, 2 = pairs only for M >= 4096 and N >= 8192
+    const int pmode = gemm_pair_mode();
+    if ((pmode == 1 && M > 256) || (pmode == 2 && M >= 4096 && N >= 8192)) {
+        p.group_m = (p.group_m + 1) / 2;  // the tile order walks m-tile PAIRS
+        const int pair_tiles = ((M + 2 * BM - 1) / (2 * BM)) * ((N + 255) / 256);
+        CUtensorMap tmA, tmBh;
+        if (make_tmap_2d_bf16(&tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, BM, BK)) return -1;
+        if (make_tmap_2d_bf16(&tmBh, W, (uint64_t)N, (uint64_t)K, (uint64_t)ldw, 128, BK)) return -1;
+        switch (epi) {
+            case EPI_PLAIN: return launch_gemm_pair<EPI_PLAIN, 256>(tmA, tmBh, p, pair_tiles, stream);
+            case EPI_RESID: return launch_gemm_pair<EPI_RESID, 256>(tmA, tmBh, p, pair_tiles, stream);
+            case EPI_F32: return launch_gemm_pair<EPI_F32, 256>(tmA, tmBh, p, pair_tiles, stream);
+            case EPI_SWIGLU: return launch_gemm_pair<EPI_SWIGLU, 256>(tmA, tmBh, p, pair_tiles, stream);
+            case EPI_QKVROPE: return launch_gemm_pair<EPI_QKVROPE, 256>(tmA, tmBh, p, pair_tiles, stream);
+            default: return set_error("gemm: unknown epilogue");
+        }
     }
     if (pl.tail > 0) {
         SkWorkspace w;
@@ -417,9 +530,6 @@ int gemm_bf16(int epi, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, 
         case EPI_SWIGLU:
             return launch_gemm<EPI_SWIGLU, 256>(tmA, tmB, p, grid, stream);
         case EPI_QKVROPE:
-            p.q = qa->q; p.k = qa->k; p.vt = qa->vt; p.cos_tab = qa->cos_tab; p.sin_tab = qa->sin_tab;
-            p.L = qa->L; p.Lpad = qa->Lpad; p.d_model = qa->d_model; p.n_heads = qa->n_heads;
-            p.pos_map = qa->pos_map; p.Tq = qa->Tq; p.row0 = qa->row0;
             return launch_gemm<EPI_QKVROPE, 256>(tmA, tmB, p, grid, stream);
         default:
             return set_error("gemm: unknown epilogue");

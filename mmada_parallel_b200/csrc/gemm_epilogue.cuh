@@ -1,5 +1,5 @@
-// Fused epilogues of the bf16 GEMM kernels (shared by the 1-CTA kernel in gemm.cu and the CTA-pair kernel in gemm2.cu).
-// One call handles one thread's row of one 128 x BN accumulator tile held in TMEM.
+// Fused epilogues of the bf16 GEMM kernel (gemm.cu). One call handles one thread's wgmma fragment of a 128 x BN
+// accumulator tile held in registers.
 #pragma once
 #include "mmdp_internal.h"
 #include "ptx.cuh"
@@ -27,8 +27,8 @@ struct GemmParams {
     int row0;  // QKVROPE: sequence index of GEMM row 0 (row-chunked launches); q / k are addressed relative to it, positions and V^T absolutely
     // split-K tail (gemm.cu): the last `sk_tail` tiles (a partial wave) are split along K into `sk_splits` (<= 8) units of
     // `sk_kb_per` k-blocks; partial accumulators meet in `sk_ws` (fp32, [tail][splits][BN/4][128] float4: column-group major,
-    // tile row minor, so that both the publishing threads (thread = row) and the finishing threads (consecutive threads =
-    // consecutive rows) touch contiguous 16-byte pieces), `sk_cnt[2*tile]` counts arrivals
+    // tile row minor, so that the finishing threads (consecutive threads = consecutive rows) read contiguous 16-byte
+    // pieces), `sk_cnt[2*tile]` counts arrivals
     int sk_tail, sk_splits, sk_kb_per;
     float* sk_ws;
     int* sk_cnt;
@@ -36,19 +36,12 @@ struct GemmParams {
     int l2pf, l2pf_mod;
     // EPI_F32 scatter (tensor parallel, GEMM fused with the reduce-scatter): scat_R > 0 -> the fp32 partial row `row` is
     // not stored to C but PUSHED over NVLink into its owner's receive buffer, scat_dst[row / scat_R] (peer-mapped,
-    // [n_ranks][scat_R][ldc] fp32), slot scat_slot = this rank; rows staged through shared memory so that every store
-    // instruction writes whole 128-byte lines
+    // [n_ranks][scat_R][ldc] fp32), slot scat_slot = this rank
     float* scat_dst[8];
     int scat_R, scat_slot;
     // tile order: group_m == 0 -> M-fastest over all m-tiles; > 0 -> M-fastest inside groups of group_m m-tiles, all n-tiles
     // of a group before the next group (keeps the group's A rows L2-resident while the weights stream)
     int group_m;
-    // CTA-pair kernel: number of tiles of the partial last wave that are cut into two half-width units (gemm2.cu)
-    int nsplit_tail;
-    // CTA-pair kernel, SwiGLU epilogue: M % 256 <= 128 -> the last m-block runs as 128-row "half-M" units (cta_group::2 MMAs with
-    // M = 128, 64 rows per CTA, half the cycles of a 256-row tile). Inside the num_m units of n-tile g the half unit sits at
-    // position (g / mt_period) % num_m so that the round-robin unit -> cluster map hands every cluster its share of them.
-    int mtail, mt_period;
 };
 
 __host__ __device__ __forceinline__ void gemm_tile_coords(int tl, int num_m, int num_n, int group_m, int& m_blk, int& n_blk) {
@@ -65,205 +58,122 @@ __host__ __device__ __forceinline__ void gemm_tile_coords(int tl, int num_m, int
     }
 }
 
-__device__ __forceinline__ void store_bf16x32(__nv_bfloat16* dst, const uint32_t (&p)[16], int ncols_valid) {
-    // dst is 16-B aligned when ldc % 8 == 0 and column offsets are multiples of 8
-    uint4* d4 = reinterpret_cast<uint4*>(dst);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        if (i * 8 < ncols_valid) d4[i] = make_uint4(p[4 * i], p[4 * i + 1], p[4 * i + 2], p[4 * i + 3]);
-    }
-}
-
-// SwiGLU of 32 (gate, up) column pairs of one row, rounding points of modeling_llada.py:962-967, stored as 32 bf16
-__device__ __forceinline__ void swiglu_store32(const GemmParams& p, const uint32_t (&g)[32], const uint32_t (&u)[32], int row, bool row_ok, int col0) {
-    const int nvalid = p.N / 2 - col0;
-    if (row_ok && nvalid > 0) {
-        uint32_t pk[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-            float o[2];
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                float gg = bf16_round(__uint_as_float(g[2 * i + h]));
-                float uu = bf16_round(__uint_as_float(u[2 * i + h]));
-                float s = bf16_round(__fdiv_rn(gg, __fadd_rn(1.0f, expf(-gg))));  // silu -> bf16
-                o[h] = __fmul_rn(s, uu);
-            }
-            pk[i] = pack_bf16x2(o[0], o[1]);
-        }
-        store_bf16x32(p.C + (size_t)row * p.ldc + col0, pk, nvalid);
-    }
-}
-
-// tbase: TMEM address of this warp's lane quarter and accumulator stage; row: global output row of this thread;
-// n_blk: N-tile index (tile columns [n_blk*BN, n_blk*BN + BN)).
-static constexpr int kScatStageFloats = 32 * 36;  // per epilogue warp: 32 rows x 32 columns, row stride 36 floats (bank-conflict free)
-
+// One thread's share of a 128 x BN accumulator tile (gemm.cu): the wgmma fragment of its warpgroup's 64-row half,
+// acc[4j + 2h + e] = tile row rit0 + 8h, tile column 8j + c0 + e (c0 = 2 * (lane % 4)). Every element goes through the
+// same rounding points as the reference; only the mapping of elements to threads is the fragment's.
 template <int EPI, int BN>
-__device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, uint32_t tbase, int row, bool row_ok, int n_blk,
-                                                   float* stage = nullptr) {
-            const int n0 = n_blk * BN;
-            if constexpr (EPI == EPI_F32) {
-              if (p.scat_R > 0) {
-                // fused reduce-scatter: push this tile's partial rows to the ranks that own them
-                const int lane = threadIdx.x & 31;
-                const int row0 = row - lane;  // first row of this warp's 32 accumulator lanes
-#pragma unroll 1
-                for (int c = 0; c < BN / 32; ++c) {
-                    uint32_t v[32];
-                    tmem_ld_32x32b_x32(tbase + c * 32, v);
-                    tmem_ld_wait();
+__device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const float (&acc)[BN / 2], int m_blk, int n_blk, int rit0,
+                                                   int c0) {
+    const int n0 = n_blk * BN;
 #pragma unroll
-                    for (int i = 0; i < 8; ++i)
-                        *reinterpret_cast<uint4*>(stage + lane * 36 + i * 4) = make_uint4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-                    __syncwarp();
-                    const int col = n0 + c * 32 + (lane & 7) * 4;
+    for (int h = 0; h < 2; ++h) {
+        const int row = m_blk * 128 + rit0 + 8 * h;
+        if (row >= p.M) continue;
+        if constexpr (EPI == EPI_F32) {
+            // raw fp32 accumulators (tensor-parallel partial sums: reduced across ranks in fp32, rounded once afterwards);
+            // scat_R > 0: the row is pushed to the receive buffer of the rank that owns it (fused reduce-scatter)
+            float* dst;
+            if (p.scat_R > 0) {
+                const int owner = row / p.scat_R;
+                dst = p.scat_dst[owner] + ((size_t)p.scat_slot * p.scat_R + (row - owner * p.scat_R)) * p.ldc;
+            } else {
+                dst = reinterpret_cast<float*>(p.C) + (size_t)row * p.ldc;
+            }
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const int r = j * 4 + (lane >> 3), grow = row0 + r;
-                        if (grow < p.M && col < p.N) {
-                            const int owner = grow / p.scat_R;
-                            float* dst = p.scat_dst[owner] + ((size_t)p.scat_slot * p.scat_R + (grow - owner * p.scat_R)) * p.ldc + col;
-                            *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(stage + r * 36 + (lane & 7) * 4);
-                        }
-                    }
-                    __syncwarp();
-                }
-              } else {
-                // raw fp32 accumulators (tensor-parallel partial sums: reduced across ranks in fp32, rounded once afterwards)
-                float* Cf = reinterpret_cast<float*>(p.C);
-#pragma unroll 1
-                for (int c = 0; c < BN / 32; ++c) {
-                    uint32_t v[32];
-                    tmem_ld_32x32b_x32(tbase + c * 32, v);
-                    tmem_ld_wait();
-                    const int col0 = n0 + c * 32;
-                    const int nvalid = p.N - col0;
-                    if (row_ok && nvalid > 0) {
-                        uint4* d4 = reinterpret_cast<uint4*>(Cf + (size_t)row * p.ldc + col0);
+            for (int j = 0; j < BN / 8; ++j) {
+                const int col = n0 + 8 * j + c0;
+                if (col < p.N) *reinterpret_cast<float2*>(dst + col) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+            }
+        } else if constexpr (EPI == EPI_PLAIN || EPI == EPI_RESID) {
 #pragma unroll
-                        for (int i = 0; i < 8; ++i)
-                            if (i * 4 < nvalid) d4[i] = make_uint4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-                    }
-                }
-              }
-            } else if constexpr (EPI == EPI_PLAIN || EPI == EPI_RESID) {
-#pragma unroll 1
-                for (int c = 0; c < BN / 32; ++c) {
-                    uint32_t v[32];
-                    tmem_ld_32x32b_x32(tbase + c * 32, v);
-                    tmem_ld_wait();
-                    const int col0 = n0 + c * 32;
-                    const int nvalid = p.N - col0;
-                    if (row_ok && nvalid > 0) {
-                        uint32_t pk[16];
-                        if constexpr (EPI == EPI_RESID) {
-                            const uint4* r4 = reinterpret_cast<const uint4*>(p.resid + (size_t)row * p.ldr + col0);
-                            uint32_t rr[16];
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) {
-                                uint4 t = (i * 8 < nvalid) ? r4[i] : make_uint4(0, 0, 0, 0);
-                                rr[4 * i] = t.x; rr[4 * i + 1] = t.y; rr[4 * i + 2] = t.z; rr[4 * i + 3] = t.w;
-                            }
-#pragma unroll
-                            for (int i = 0; i < 16; ++i) {
-                                // nn.Linear output is rounded to bf16 first, then the residual add rounds again
-                                float a0 = bf16_round(__uint_as_float(v[2 * i]));
-                                float a1 = bf16_round(__uint_as_float(v[2 * i + 1]));
-                                pk[i] = pack_bf16x2(__fadd_rn(bf16_lo(rr[i]), a0), __fadd_rn(bf16_hi(rr[i]), a1));
-                            }
-                        } else {
-#pragma unroll
-                            for (int i = 0; i < 16; ++i)
-                                pk[i] = pack_bf16x2(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1]));
-                        }
-                        store_bf16x32(p.C + (size_t)row * p.ldc + col0, pk, nvalid);
-                    }
-                }
-            } else if constexpr (EPI == EPI_SWIGLU) {
-                // tile columns [0,128) = gate rows of W1, [128,256) = up rows of W3 (weights packed interleaved)
-#pragma unroll 1
-                for (int c = 0; c < 4; ++c) {
-                    uint32_t g[32], u[32];
-                    tmem_ld_32x32b_x32(tbase + c * 32, g);
-                    tmem_ld_32x32b_x32(tbase + 128 + c * 32, u);
-                    tmem_ld_wait();
-                    swiglu_store32(p, g, u, row, row_ok, n_blk * 128 + c * 32);
-                }
-            } else if constexpr (EPI == EPI_QKVROPE) {
-                const int region = n0 / p.d_model;  // 0 = Q, 1 = K, 2 = V (d_model % 256 == 0 is checked on the host)
-                int b, pos;
-                if (p.pos_map) {
-                    b = row_ok ? row / p.Tq : 0;
-                    pos = row_ok ? p.pos_map[row] : 0;
+            for (int j = 0; j < BN / 8; ++j) {
+                const int col = n0 + 8 * j + c0;
+                if (col >= p.N) continue;
+                const float a0 = acc[4 * j + 2 * h], a1 = acc[4 * j + 2 * h + 1];
+                uint32_t o;
+                if constexpr (EPI == EPI_RESID) {
+                    // nn.Linear output is rounded to bf16 first, then the residual add rounds again
+                    const uint32_t rr = *reinterpret_cast<const uint32_t*>(p.resid + (size_t)row * p.ldr + col);
+                    o = pack_bf16x2(__fadd_rn(bf16_lo(rr), bf16_round(a0)), __fadd_rn(bf16_hi(rr), bf16_round(a1)));
                 } else {
-                    b = row_ok ? (row + p.row0) / p.L : 0;
-                    pos = row_ok ? (row + p.row0) - b * p.L : 0;
+                    o = pack_bf16x2(a0, a1);
                 }
-                if (region < 2) {
-                    const size_t drow = (region == 0 || !p.pos_map) ? (size_t)row : (size_t)b * p.L + pos;  // k rows go to their sequence position
-                    __nv_bfloat16* dst = (region == 0 ? p.q : p.k) + drow * p.d_model + (n0 - region * p.d_model);
-#pragma unroll 1
-                    for (int hc = 0; hc < BN / 64; ++hc) {  // (head in tile) x (32-col chunk of the first half)
-                        const int head = hc >> 1, cc = hc & 1;
-                        uint32_t x1[32], x2[32];
-                        tmem_ld_32x32b_x32(tbase + head * 128 + cc * 32, x1);
-                        tmem_ld_32x32b_x32(tbase + head * 128 + 64 + cc * 32, x2);
-                        tmem_ld_wait();
-                        if (row_ok) {
-                            const float4* c4 = reinterpret_cast<const float4*>(p.cos_tab + (size_t)pos * 64 + cc * 32);
-                            const float4* s4 = reinterpret_cast<const float4*>(p.sin_tab + (size_t)pos * 64 + cc * 32);
-                            uint32_t o1[16], o2[16];
+                *reinterpret_cast<uint32_t*>(p.C + (size_t)row * p.ldc + col) = o;
+            }
+        } else if constexpr (EPI == EPI_SWIGLU) {
+            // tile columns [0,128) = gate rows of W1, [128,256) = up rows of W3 (weights packed interleaved)
 #pragma unroll
-                            for (int i = 0; i < 8; ++i) {
-                                const float4 cv = c4[i], sv = s4[i];
-                                const float cs[4] = {cv.x, cv.y, cv.z, cv.w};
-                                const float sn[4] = {sv.x, sv.y, sv.z, sv.w};
-                                float a[4], bb[4];
+            for (int j = 0; j < 16; ++j) {
+                const int col = n_blk * 128 + 8 * j + c0;
+                if (col >= p.N / 2) continue;
+                float o[2];
 #pragma unroll
-                                for (int j = 0; j < 4; ++j) {
-                                    const float t1 = bf16_round(__uint_as_float(x1[4 * i + j]));
-                                    const float t2 = bf16_round(__uint_as_float(x2[4 * i + j]));
-                                    // (t * cos) + (rotate_half(t) * sin), fp32, no FMA contraction
-                                    a[j] = __fadd_rn(__fmul_rn(t1, cs[j]), __fmul_rn(-t2, sn[j]));
-                                    bb[j] = __fadd_rn(__fmul_rn(t2, cs[j]), __fmul_rn(t1, sn[j]));
-                                }
-                                o1[2 * i] = pack_bf16x2(a[0], a[1]);
-                                o1[2 * i + 1] = pack_bf16x2(a[2], a[3]);
-                                o2[2 * i] = pack_bf16x2(bb[0], bb[1]);
-                                o2[2 * i + 1] = pack_bf16x2(bb[2], bb[3]);
-                            }
-                            store_bf16x32(dst + head * 128 + cc * 32, o1, 32);
-                            store_bf16x32(dst + head * 128 + 64 + cc * 32, o2, 32);
+                for (int e = 0; e < 2; ++e) {
+                    const float gg = bf16_round(acc[4 * j + 2 * h + e]);
+                    const float uu = bf16_round(acc[4 * (j + 16) + 2 * h + e]);
+                    const float s = bf16_round(__fdiv_rn(gg, __fadd_rn(1.0f, expf(-gg))));  // silu -> bf16
+                    o[e] = __fmul_rn(s, uu);
+                }
+                *reinterpret_cast<uint32_t*>(p.C + (size_t)row * p.ldc + col) = pack_bf16x2(o[0], o[1]);
+            }
+        } else if constexpr (EPI == EPI_QKVROPE) {
+            const int region = n0 / p.d_model;  // 0 = Q, 1 = K, 2 = V (d_model % 256 == 0 is checked on the host)
+            int b, pos;
+            if (p.pos_map) {
+                b = row / p.Tq;
+                pos = p.pos_map[row];
+            } else {
+                b = (row + p.row0) / p.L;
+                pos = (row + p.row0) - b * p.L;
+            }
+            if (region < 2) {
+                const size_t drow = (region == 0 || !p.pos_map) ? (size_t)row : (size_t)b * p.L + pos;  // k rows go to their sequence position
+                __nv_bfloat16* dst = (region == 0 ? p.q : p.k) + drow * p.d_model + (n0 - region * p.d_model);
+#pragma unroll
+                for (int head = 0; head < BN / 128; ++head) {
+#pragma unroll
+                    for (int jj = 0; jj < 8; ++jj) {  // columns c and c + 64 of the head: the rotary pair
+                        const int j = head * 16 + jj, c = 8 * jj + c0;
+                        const float2 cs = *reinterpret_cast<const float2*>(p.cos_tab + (size_t)pos * 64 + c);
+                        const float2 sn = *reinterpret_cast<const float2*>(p.sin_tab + (size_t)pos * 64 + c);
+                        const float csv[2] = {cs.x, cs.y}, snv[2] = {sn.x, sn.y};
+                        float a[2], bb[2];
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const float t1 = bf16_round(acc[4 * j + 2 * h + e]);
+                            const float t2 = bf16_round(acc[4 * (j + 8) + 2 * h + e]);
+                            // (t * cos) + (rotate_half(t) * sin), fp32, no FMA contraction
+                            a[e] = __fadd_rn(__fmul_rn(t1, csv[e]), __fmul_rn(-t2, snv[e]));
+                            bb[e] = __fadd_rn(__fmul_rn(t2, csv[e]), __fmul_rn(t1, snv[e]));
                         }
+                        *reinterpret_cast<uint32_t*>(dst + head * 128 + c) = pack_bf16x2(a[0], a[1]);
+                        *reinterpret_cast<uint32_t*>(dst + head * 128 + 64 + c) = pack_bf16x2(bb[0], bb[1]);
                     }
-                } else {
-                    // V is written transposed: vt[b][head][d][token] so that P·V runs with both operands K-major
-#pragma unroll 1
-                    for (int c = 0; c < BN / 32; ++c) {
-                        uint32_t v[32];
-                        tmem_ld_32x32b_x32(tbase + c * 32, v);
-                        tmem_ld_wait();
-                        if (row_ok) {
-                            const int n = n0 - 2 * p.d_model + c * 32;
-                            const int head = n >> 7, d0 = n & 127;
-                            __nv_bfloat16* dst = p.vt + ((size_t)(b * p.n_heads + head) * 128 + d0) * p.Lpad + pos;
+                }
+            } else {
+                // V is written transposed: vt[b][head][d][token] so that P·V runs with both operands K-major
 #pragma unroll
-                            for (int i = 0; i < 32; ++i) dst[(size_t)i * p.Lpad] = __float2bfloat16_rn(__uint_as_float(v[i]));
-                        }
-                    }
+                for (int j = 0; j < BN / 8; ++j) {
+                    const int n = n0 - 2 * p.d_model + 8 * j + c0;
+                    const int head = n >> 7, d0 = n & 127;
+                    __nv_bfloat16* dst = p.vt + ((size_t)(b * p.n_heads + head) * 128 + d0) * p.Lpad + pos;
+                    dst[0] = __float2bfloat16_rn(acc[4 * j + 2 * h]);
+                    dst[p.Lpad] = __float2bfloat16_rn(acc[4 * j + 2 * h + 1]);
                 }
             }
+        }
+    }
 }
 
 // ------------------------------------------------------------------------------------------------------------------
 // Split-K tail: finishing pass. The S units of a tail tile have published their fp32 partial accumulators in the
-// workspace; unit `s` owns the tile rows [128*s/S, 128*(s+1)/S) and, with all 128 epilogue threads, sums the partials of
+// workspace; unit `s` owns the tile rows [128*s/S, 128*(s+1)/S) and, with all kEpiThreads epilogue threads, sums the partials of
 // those rows in split order 0..S-1 (fixed -> deterministic; every load of an item is in flight before the first add) and
 // applies the ordinary fused epilogue. Work items are (row, 8-column group) - for the rotary / SwiGLU epilogues the
 // group's partner columns (+64 / +128) are fetched with it - and consecutive threads take consecutive rows of one group.
 // ------------------------------------------------------------------------------------------------------------------
 static constexpr int kSkMaxSplits = 8;
+static constexpr int kEpiThreads = 256;  // the two MMA warpgroups of gemm.cu run the finishing pass
 
 template <int BN, int NV>
 __device__ __forceinline__ void sk_sum(const float4* __restrict__ tile_ws, int S, int row, const int (&col4)[NV], float4 (&acc)[NV]) {
@@ -299,19 +209,17 @@ __device__ __forceinline__ void sk_sum(const float4* __restrict__ tile_ws, int S
     }
 }
 
-// publish this thread's accumulator row (TMEM lane `rit`) into split slot `slot_ws` ([BN/4][128] float4)
+// publish this thread's accumulator fragment into split slot `slot_ws` ([BN/4][128] float4, viewed as floats)
 template <int BN>
-__device__ __forceinline__ void sk_publish(float4* __restrict__ slot_ws, uint32_t tbase, int rit) {
-#pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tbase + c * 32, v);
-        tmem_ld_wait();
+__device__ __forceinline__ void sk_publish(float* __restrict__ slot_ws, const float (&acc)[BN / 2], int rit0, int c0) {
 #pragma unroll
-        for (int i = 0; i < 8; ++i)
-            slot_ws[(size_t)(c * 8 + i) * 128 + rit] = make_float4(__uint_as_float(v[4 * i]), __uint_as_float(v[4 * i + 1]),
-                                                                  __uint_as_float(v[4 * i + 2]), __uint_as_float(v[4 * i + 3]));
-    }
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+            const int col = 8 * j + c0;
+            *reinterpret_cast<float2*>(slot_ws + ((size_t)(col >> 2) * 128 + rit0 + 8 * h) * 4 + (col & 3)) =
+                make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        }
 }
 
 template <int EPI, int BN>
@@ -322,7 +230,7 @@ __device__ __forceinline__ void sk_finish(const GemmParams& p, const float4* __r
     const int n0 = n_blk * BN;
     if constexpr (EPI == EPI_PLAIN || EPI == EPI_RESID || EPI == EPI_F32) {
         constexpr int G = BN / 8;
-        for (int idx = tid; idx < nrows * G; idx += 128) {
+        for (int idx = tid; idx < nrows * G; idx += kEpiThreads) {
             const int g = idx / nrows, rit = r0 + idx - g * nrows;
             const int row = m_blk * 128 + rit, col = n0 + 8 * g;
             if (row >= p.M || col >= p.N) continue;
@@ -351,7 +259,7 @@ __device__ __forceinline__ void sk_finish(const GemmParams& p, const float4* __r
         }
     } else if constexpr (EPI == EPI_SWIGLU) {
         constexpr int G = 16;  // 128 output columns per tile
-        for (int idx = tid; idx < nrows * G; idx += 128) {
+        for (int idx = tid; idx < nrows * G; idx += kEpiThreads) {
             const int g = idx / nrows, rit = r0 + idx - g * nrows;
             const int row = m_blk * 128 + rit, col = n_blk * 128 + 8 * g;
             if (row >= p.M || col >= p.N / 2) continue;
@@ -375,7 +283,7 @@ __device__ __forceinline__ void sk_finish(const GemmParams& p, const float4* __r
         if (region < 2) {
             constexpr int G = 16;  // 2 heads x 8 column groups of the first half
             __nv_bfloat16* base = (region == 0 ? p.q : p.k) + (n0 - region * p.d_model);
-            for (int idx = tid; idx < nrows * G; idx += 128) {
+            for (int idx = tid; idx < nrows * G; idx += kEpiThreads) {
                 const int g = idx / nrows, rit = r0 + idx - g * nrows;
                 const int row = m_blk * 128 + rit;
                 if (row >= p.M) continue;
@@ -406,7 +314,7 @@ __device__ __forceinline__ void sk_finish(const GemmParams& p, const float4* __r
             }
         } else {
             constexpr int G = BN / 8;
-            for (int idx = tid; idx < nrows * G; idx += 128) {
+            for (int idx = tid; idx < nrows * G; idx += kEpiThreads) {
                 const int g = idx / nrows, rit = r0 + idx - g * nrows;
                 const int row = m_blk * 128 + rit;
                 if (row >= p.M) continue;

@@ -33,8 +33,8 @@ int pdl_mode();
 void set_pdl_mode(int on);
 int env_int(const char* name, int dflt);
 // tuning options (runtime.cu): environment default, mmdp_set_option(key, value) at run time
-enum OptId { OPT_PDL = 0, OPT_GEMM_SPLITK, OPT_GEMM_L2PF, OPT_GEMM_L2PF_MOD, OPT_GEMM_PAIR, OPT_GEMM_GROUP_M, OPT_ATTN_SPLIT_TAIL,
-             OPT_ATTN_POLY, OPT_RMSNORM_WARP, OPT_GEMM_NSPLIT_TAIL, OPT_ATTN_VERSION, OPT_ATTN_PROBE, OPT_GEMM_MTAIL, OPT_ROW_WINDOW, OPT_COUNT };
+enum OptId { OPT_PDL = 0, OPT_GEMM_SPLITK, OPT_GEMM_L2PF, OPT_GEMM_L2PF_MOD, OPT_GEMM_GROUP_M, OPT_ATTN_SPLIT_TAIL,
+             OPT_RMSNORM_WARP, OPT_ROW_WINDOW, OPT_ATTN_VERSION, OPT_GEMM_PAIR, OPT_COUNT };
 int opt(int id);
 int set_opt(const char* key, int value);
 
@@ -117,10 +117,6 @@ int gemm_bf16(int epi, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, 
               __nv_bfloat16* C, int ldc, const __nv_bfloat16* resid, int ldr, const QkvRopeArgs* qa,
               cudaStream_t stream, const GemmScatter* sc = nullptr);
 
-// CTA-pair (cta_group::2) kernel, gemm2.cu; selected by MMDP_GEMM_PAIR=1 or mmdp_set_gemm_pair(1)
-int gemm_bf16_pair(int epi, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int ldw, int M, int N, int K,
-                   __nv_bfloat16* C, int ldc, const __nv_bfloat16* resid, int ldr, const QkvRopeArgs* qa, cudaStream_t stream,
-                   const GemmScatter* sc = nullptr);
 int gemm_pair_mode();
 void set_gemm_pair_mode(int on);
 int gemm_splitk_mode();

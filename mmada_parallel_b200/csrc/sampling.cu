@@ -108,8 +108,8 @@ __global__ void __launch_bounds__(kThreads) text_rows_kernel(TextRowArgs a) {
         if (threadIdx.x != 0) best_i = 0x7fffffff;
     } else
     for (int i0 = threadIdx.x; i0 < nvec; i0 += 4 * kThreads) {
-        // four independent 16-byte loads per tensor in flight per thread (ncu, profiles/r02: one CTA of 16 warps per SM left the
-        // kernel latency-bound at 7 % of DRAM throughput)
+        // four independent 16-byte loads per tensor in flight per thread (with one load at a time, one CTA of 16 warps per SM
+        // leaves the kernel latency-bound)
         uint4 cv[4], uv[4], nv[4];
 #pragma unroll
         for (int t = 0; t < 4; ++t) {

@@ -55,7 +55,7 @@ def generate_image(
     _trace: Optional[list] = None,
 ) -> torch.LongTensor:
     if not hasattr(model, "forward_rows"):
-        raise TypeError("generate_image needs a mmada_parallel_b200.model.LLaDAForMultiModalGeneration (B200-native) model")
+        raise TypeError("generate_image needs a mmada_parallel_b200.model.LLaDAForMultiModalGeneration (H100-native) model")
     if debug and debug_log_dir:
         os.makedirs(debug_log_dir, exist_ok=True)
     device = model.device

@@ -236,7 +236,7 @@ def generate_ti2ti(
         # 'random' requests int64 uniform noise in the reference and raises there too (:195-197)
         raise NotImplementedError(remasking)
     if not hasattr(model, "forward_rows"):
-        raise TypeError("generate_ti2ti needs a mmada_parallel_b200.model.LLaDAForMultiModalGeneration (B200-native) model")
+        raise TypeError("generate_ti2ti needs a mmada_parallel_b200.model.LLaDAForMultiModalGeneration (H100-native) model")
     if input_ids.shape[0] != 1:
         raise ValueError("the image path of generate_ti2ti is single-sample (reference :224/:340 read batch row 0 only)")
     ids_host = input_ids.detach().to("cpu", torch.int64)

@@ -58,7 +58,7 @@ def generate_ti2ti_stepwise(
     if remasking != "low_confidence":
         raise NotImplementedError(remasking)
     if not hasattr(model, "forward_rows"):
-        raise TypeError("generate_ti2ti_stepwise needs a mmada_parallel_b200.model.LLaDAForMultiModalGeneration (B200-native) model")
+        raise TypeError("generate_ti2ti_stepwise needs a mmada_parallel_b200.model.LLaDAForMultiModalGeneration (H100-native) model")
     if input_ids.shape[0] != 1:
         raise ValueError("the image path is single-sample (the reference reads batch row 0 only, app.py:199/:300)")
     ids_host = input_ids.detach().to("cpu", torch.int64)

@@ -1,6 +1,6 @@
 """Drop-in for the decode side of MMaDA-Parallel-M/models/modeling_magvitv2.py: `MAGVITv2.decode_code`
 (:429-433) = LFQuantizer.get_codebook_entry (:208-221) + VQGANDecoder.forward (:365-399), as one C call into the native
-decoder context (TF32 tcgen05 implicit-GEMM convolutions, csrc/conv_tf32.cu + csrc/vq_decoder.cu).
+decoder context (TF32 wgmma implicit-GEMM convolutions, csrc/conv_tf32.cu + csrc/vq_decoder.cu).
 
 Numerics: the reference module runs in fp32; on a GPU its convolutions go through cuDNN with TF32 allowed (PyTorch
 default), which is the precision of this implementation (10-bit mantissa products, fp32 accumulation). Tolerance against
@@ -22,7 +22,7 @@ class VQGANDecoder:
     def __init__(self, ch: int = 128, ch_mult: Sequence[int] = (1, 1, 2, 2, 4), num_res_blocks: Sequence[int] = (4, 4, 3, 4, 3),
                  z_channels: int = 13, out_ch: int = 3, latent_hw=(32, 32), max_batch: int = 1, device: str = "cuda:0"):
         if not torch.cuda.is_available():
-            raise _lib.MmdpError("mmada_parallel_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise _lib.MmdpError("mmada_parallel_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device(device)
         torch.cuda.set_device(self.device)
         self.cfg = SimpleNamespace(ch=ch, ch_mult=tuple(ch_mult), num_res_blocks=tuple(num_res_blocks), z_channels=z_channels,
@@ -116,7 +116,7 @@ class VQGANEncoder:
     def __init__(self, ch: int = 128, ch_mult: Sequence[int] = (1, 2, 2, 4, 4), num_res_blocks: Sequence[int] = (4, 3, 4, 3, 4),
                  z_channels: int = 13, in_ch: int = 3, latent_hw=(32, 32), max_batch: int = 1, device: str = "cuda:0"):
         if not torch.cuda.is_available():
-            raise _lib.MmdpError("mmada_parallel_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise _lib.MmdpError("mmada_parallel_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device(device)
         torch.cuda.set_device(self.device)
         c = _lib.VqDecConfig()

@@ -3,7 +3,7 @@
 `LLaDAForMultiModalGeneration` keeps the call contract of the reference wrapper
 (MMaDA-Parallel-A/model/modeling_xllmx_dimoo.py:41-72): ``model(input_ids, infer=True, use_cache=False).logits``
 returns bf16 logits ``[B, L, V]`` on ``model.device``. Underneath, weights live in device buffers owned by the native
-context (libmmdp.so, include/mmdp.h) and one forward is a single C call that launches the sm_100a kernels.
+context (libmmdp.so, include/mmdp.h) and one forward is a single C call that launches the sm_90a kernels.
 
 The same object also exposes ``forward_rows`` - the restricted LM head the generators use so the full ``[L, V]``
 logits never hit HBM (only text rows x V and image rows x codebook columns are computed).
@@ -48,7 +48,7 @@ def check_supported_config(config, n_heads: int) -> None:
     for flag in ("alibi", "include_bias", "include_qkv_bias", "weight_tying", "scale_logits", "input_emb_norm",
                  "attention_layer_norm"):
         if g(flag, False):
-            raise NotImplementedError(f"config.{flag}=True is not supported by the B200 hot path")
+            raise NotImplementedError(f"config.{flag}=True is not supported by the H100 hot path")
     if not g("rope", True) or not g("rope_full_precision", True):
         raise NotImplementedError("the hot path implements full-precision RoPE only")
     # the kernels implement LLaDALlamaBlock + SwiGLU(silu) + RMSLayerNorm only (modeling_llada.py:906-972, :315-329);
@@ -57,16 +57,16 @@ def check_supported_config(config, n_heads: int) -> None:
         v = g(key, None)
         v = getattr(v, "value", v)  # the reference uses StrEnum members
         if v is not None and str(v).lower() not in ok:
-            raise NotImplementedError(f"config.{key}={v!r} is not supported by the B200 hot path (needs one of {ok})")
+            raise NotImplementedError(f"config.{key}={v!r} is not supported by the H100 hot path (needs one of {ok})")
 
 
 class LLaDAForMultiModalGeneration:
-    """B200-native drop-in for the reference's inference-time model object (variant A wrapper and, through
+    """H100-native drop-in for the reference's inference-time model object (variant A wrapper and, through
     `MMadaModelLM` in mmada.py, variant M)."""
 
     def __init__(self, config, max_seq_len: Optional[int] = None, max_batch: int = 3, device: str = "cuda:0"):
         if not torch.cuda.is_available():
-            raise _lib.MmdpError("mmada_parallel_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise _lib.MmdpError("mmada_parallel_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.config = config
         self.device = torch.device(device)
         torch.cuda.set_device(self.device)
@@ -263,7 +263,7 @@ class LLaDAForMultiModalGeneration:
         extra keywords are those of the class underneath it, LLaDAModelLM.forward (modeling_llada.py:1475-1477): with the token
         cache switched on (`caching(True)`) and `use_cache=True` they select the partial-recompute forward."""
         if labels is not None or not infer:
-            raise NotImplementedError("only the inference branch (infer=True) is on the B200 hot path")
+            raise NotImplementedError("only the inference branch (infer=True) is on the H100 hot path")
         if to_compute_mask is not None and not (use_cache and getattr(self, "_caching", False)):
             raise ValueError("to_compute_mask needs the token cache: model.caching(True) and use_cache=True")
         # use_cache=True with the cache switched on and no mask: a full forward that fills the caches (same logits);

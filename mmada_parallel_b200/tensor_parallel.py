@@ -139,15 +139,14 @@ class TensorParallelLLaDA:
                  max_seq_len: Optional[int] = None, max_batch: int = 1, device: str = "cuda:0", text_vocab_size: int = 126356,
                  codebook_size: int = 8192, collective: str = "p2p", chunks: Optional[int] = None):
         if not torch.cuda.is_available():
-            raise _lib.MmdpError("mmada_parallel_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise _lib.MmdpError("mmada_parallel_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         if collective not in ("p2p", "nccl"):
             raise ValueError("collective must be 'p2p' (NVLink peer-memory kernel) or 'nccl' (all-reduce baseline)")
         self.config, self.group, self.rank, self.tp = config, group, tp_rank, tp_size
         self.collective = collective if tp_size > 1 else "nccl"
         if chunks is None:
-            # measured (bench.py `tp` record, profiles/r02): two half-size chains on two streams LOSE 5 % against one chunk at both
-            # ends of the range - 306 vs 323 tokens/s at TP=2, 510 vs 538 at TP=8: the half-size GEMMs and the doubled launch
-            # count cost more than the NVLink time they hide. The schedule stays available (chunks=2, bitwise identical results).
+            # one chunk by default: two half-size chains on two streams halve the GEMMs and double the launches, which has cost more
+            # than the NVLink time they hide. The schedule stays available (chunks=2, bitwise identical results).
             chunks = 1
         if chunks not in (1, 2):
             raise ValueError("chunks must be 1 or 2")

@@ -2,7 +2,7 @@
 
 The reference decodes with the aMUSEd VQ-VAE (`diffusers.VQModel`, not part of this repository - DESIGN.md section 5); here
 the decoder is any object with the native protocol of `mmada_parallel_b200.magvit.MAGVITv2`:
-    vqvae.decode_code(ids[B, N]) -> FloatTensor[B, 3, H, W] in ~[-1, 1]      (C call into the TF32 tcgen05 decoder)
+    vqvae.decode_code(ids[B, N]) -> FloatTensor[B, 3, H, W] in ~[-1, 1]      (C call into the TF32 wgmma decoder)
     vqvae.decoder.upscale                                                     (pixels per latent cell, 16 for 5 levels)
 Same arguments, same `ValueError` on a length mismatch (:48-52), same return type (one PIL image, batch row 0).
 """

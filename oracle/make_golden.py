@@ -1,11 +1,11 @@
-"""Generates tests/golden/*.pt by running the REAL reference (imported read-only from /root/reference) on seeded
+"""Generates tests/golden/*.pt by running the REAL reference (imported read-only from MMDP_REFERENCE_ROOT) on seeded
 inputs, and checks the oracle restatement against it while doing so ("pinning the oracle").
 
     PYTHONDONTWRITEBYTECODE=1 python -m oracle.make_golden
 
-Runs only in the build container (the reference is not on the GPU box). The fixtures are small (ids, noise seeds,
+Runs only where a reference checkout is available (MMDP_REFERENCE_ROOT). The fixtures are small (ids, noise seeds,
 a few hundred logits) and are committed; tests/test_oracle_golden.py re-checks the oracle against them on every run and
-tests/test_gpu_*.py check the CUDA path against them on the B200.
+tests/test_gpu_*.py check the CUDA path against them on the H100.
 """
 from __future__ import annotations
 

@@ -1,5 +1,5 @@
-"""Pins oracle/magvit.py against the REAL MAGVITv2 decoder (imported read-only from /root/reference) and writes
-tests/golden/magvit_decode.pt. Build container only.    PYTHONDONTWRITEBYTECODE=1 python -m oracle.make_golden_magvit"""
+"""Pins oracle/magvit.py against the REAL MAGVITv2 decoder (imported read-only from MMDP_REFERENCE_ROOT) and writes
+tests/golden/magvit_decode.pt. Needs MMDP_REFERENCE_ROOT.    PYTHONDONTWRITEBYTECODE=1 python -m oracle.make_golden_magvit"""
 import contextlib
 import io
 import os

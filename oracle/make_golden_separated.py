@@ -7,8 +7,8 @@ allows"). Writes tests/golden/trajectory_a_separated.pt.
 
 Construction: the tiny LLaDA of the other fixtures, but the LM head keeps only a few LIVE rows (24 text tokens, 16 VQ codes,
 gain 4); every other row is scaled by 1e-3, so logits have a handful of well-spread candidates instead of 134 656 near-ties.
-A seed is accepted when the oracle trajectory is unchanged under 8 independent perturbations of the logits by +-3 bf16 ulp of
-the logit scale (the GPU test first checks that its logits are inside this radius of the oracle's; measured error is well below 1 ulp; dead rows are perturbed in proportion to their row
+A seed is accepted when the oracle trajectory is unchanged under N_PERTURB independent perturbations of the logits by +-3 bf16
+ulp of the logit scale (the GPU test first checks that its logits are inside this radius of the oracle's; dead rows are perturbed in proportion to their row
 norm, as accumulation error is) - every decision (argmax, top-k confidence rank, sampling race, re-mask cut) then has more than
 that margin with overwhelming probability. The accepted configuration is run through the REAL reference, which must agree
 with the unperturbed oracle, and its per-step ids are stored.
@@ -29,6 +29,8 @@ N_LIVE_TEXT, N_LIVE_VQ, GAIN, DEAD = 24, 16, 4.0, 1e-3
 RUNS = [("greedy", dict(text_steps=4, timesteps=2, text_gen_length=8, temperature=0.0, text_temperature=0.0, cfg_scale=0.0, cfg_img=4.0)),
         ("bench_like", dict(text_steps=4, timesteps=2, text_gen_length=8, temperature=1.0, text_temperature=0.0, cfg_scale=0.0, cfg_img=4.0)),
         ("both_cfg_gumbel", dict(text_steps=4, timesteps=2, text_gen_length=8, temperature=0.8, text_temperature=0.5, cfg_scale=1.5, cfg_img=3.0))]
+# 32 perturbations: with 8, a seed was accepted whose bench-like trajectory an H100 forward inside the radius still flipped
+N_PERTURB = 32
 PERTURB_ULPS = 3.0   # measured GPU error on these models: up to 2.5 bf16 ulp of the logit scale (a single bf16 rounding step of the largest logits is already 1.6); the test re-checks <= 3
 
 
@@ -83,7 +85,7 @@ def main():
             om = llada.OracleModel(cfg, sd)
             img, txt, tr = trajectory(om, lay, kw, seed=wseed + 1, global_seed=wseed + 2)
             ok = True
-            for p in range(8):
+            for p in range(N_PERTURB):
                 i2, t2, _ = trajectory(PerturbedModel(om, gain, PERTURB_ULPS, 100 * wseed + p), lay, kw, seed=wseed + 1, global_seed=wseed + 2)
                 if i2 != img or t2 != txt:
                     ok = False

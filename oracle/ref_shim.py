@@ -1,6 +1,6 @@
-"""Loader for the REAL reference (read-only import from /root/reference). Used ONLY in the build container by
-oracle/make_golden.py to pin the oracle; /root/reference does not exist on the GPU box, and nothing under tests -m gpu,
-smoke() or bench.py may import this module.
+"""Loader for the REAL reference (read-only import from the checkout named by MMDP_REFERENCE_ROOT). Used ONLY by
+oracle/make_golden*.py to pin the oracle and write the golden fixtures; nothing under tests, smoke() or bench.py may import
+this module, so the suite runs without the reference.
 
 Recipes follow SURVEY.md §8c. No reference source is copied; modules are imported where they lie, with
 PYTHONDONTWRITEBYTECODE so nothing is written into the read-only tree.
@@ -12,7 +12,7 @@ import os
 import sys
 import types
 
-REF_ROOT = os.environ.get("MMDP_REFERENCE_ROOT", "/root/reference")
+REF_ROOT = os.environ.get("MMDP_REFERENCE_ROOT", "")  # a checkout of tyfeld/MMaDA-Parallel
 REF_A = os.path.join(REF_ROOT, "MMaDA-Parallel-A")
 REF_M = os.path.join(REF_ROOT, "MMaDA-Parallel-M")
 
@@ -20,7 +20,7 @@ sys.dont_write_bytecode = True
 
 
 def available() -> bool:
-    return os.path.isdir(REF_A) and os.path.isdir(REF_M)
+    return bool(REF_ROOT) and os.path.isdir(REF_A) and os.path.isdir(REF_M)
 
 
 def load_a():

@@ -172,7 +172,7 @@ def mask_by_random_topk_a(mask_len: int, probs: torch.Tensor, temperature: float
     stable=False issues the reference's own call, torch.sort(confidence, descending=False): its order among EQUAL
     bf16 confidences is implementation-defined (on an AVX-512 CPU ATen uses an unstable SIMD sort; the CUDA backend
     orders differently again), so which of several tied tokens stays masked is not a property of the algorithm.
-    stable=True is the deterministic rule the B200 kernel implements (ties -> lower index first)."""
+    stable=True is the deterministic rule the H100 kernel implements (ties -> lower index first)."""
     if noise is None:
         noise = torch.zeros_like(probs)
     confidence = torch.log(probs + 1e-10) + temperature * noise

@@ -26,7 +26,7 @@ _TINY_CACHE = {}
 
 
 def tiny_gpu_model(meta, cls=None, max_batch=3):
-    """B200-native model with the deterministic tiny weights of the golden fixtures (cached per process)."""
+    """H100-native model with the deterministic tiny weights of the golden fixtures (cached per process)."""
     from mmada_parallel_b200.model import LLaDAForMultiModalGeneration
     cls = cls or LLaDAForMultiModalGeneration
     key = (cls.__name__, meta["weight_seed"], tuple(sorted(meta["tiny"].items())), max_batch)
@@ -41,7 +41,7 @@ def tiny_gpu_model(meta, cls=None, max_batch=3):
 
 
 class GpuBackedOracleModel:
-    """Oracle-side model whose logits come from the B200 forward (full LM head), moved to the CPU. Lets the CPU oracle
+    """Oracle-side model whose logits come from the H100 forward (full LM head), moved to the CPU. Lets the CPU oracle
     loop run on exactly the logits the CUDA sampling kernels see, so integer decisions must agree bit-for-bit."""
 
     def __init__(self, gpu_model):

@@ -1,5 +1,5 @@
 // Host-side check (no GPU needed) of the GEMM tile order: gemm_tile_coords must be a bijection of [0, num_m * num_n) onto the
-// tile grid for every group size, and a wave of 148 consecutive tiles of the grouped order must span fewer m-tiles.
+// tile grid for every group size, and a wave of 132 consecutive tiles (one per H100 SM) of the grouped order must span fewer m-tiles.
 // Built and run by tests/test_host_logic.py with nvcc (host code only).
 #include <cstdio>
 #include <vector>
@@ -23,10 +23,10 @@ int main() {
             }
         }
     }
-    // wave shape at the bench-adjacent shape: 57 m-tiles x 48 n-tiles, first wave of 148 tiles
+    // wave shape at the bench-adjacent shape: 57 m-tiles x 48 n-tiles, first wave of 132 tiles
     auto span = [](int g) {
         int mmin = 1 << 30, mmax = -1;
-        for (int tl = 0; tl < 148; ++tl) { int m, n; mmdp::gemm_tile_coords(tl, 57, 48, g, m, n); mmin = m < mmin ? m : mmin; mmax = m > mmax ? m : mmax; }
+        for (int tl = 0; tl < 132; ++tl) { int m, n; mmdp::gemm_tile_coords(tl, 57, 48, g, m, n); mmin = m < mmin ? m : mmin; mmax = m > mmax ? m : mmax; }
         return mmax - mmin + 1;
     };
     if (span(0) != 57 || span(29) != 29) { printf("FAIL wave span %d %d\n", span(0), span(29)); return 1; }

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM / attention / norm kernels against fp32 torch references of the same op (floating-point kernels).
+"""wgmma GEMM / attention / norm kernels against fp32 torch references of the same op (floating-point kernels).
 Tolerances: the outputs are bf16 roundings of fp32-accumulated results; a different accumulation order may move a value
 across one rounding boundary, so the bound is 1 bf16 ulp of the result magnitude per bf16 rounding point on the path
 (2 for the residual epilogue, 3 for SwiGLU), stated per test."""
@@ -47,7 +47,6 @@ def test_gemm_grouped_tile_order(M):
     residual epilogues (the latter with its split-K tail) against the fp32 reference, and bit-identical to the plain order."""
     import os
     from mmada_parallel_b200 import _lib
-    _lib.lib.mmdp_set_gemm_pair(0)
     torch.manual_seed(M)
     K, N = 512, 1024
     a = bf(torch.randn(M, K, device="cuda") * 0.5)
@@ -58,7 +57,6 @@ def test_gemm_grouped_tile_order(M):
     assert_ulp(got, lin, 1, f"grouped gemm {M}")
     assert_ulp(_lib.gemm_bf16(a, w, _lib.EPI_RESID, resid=r), bf(lin.float() + r.float()), 2, f"grouped resid {M}", mag=lin)
     assert torch.equal(got, _lib.gemm_bf16(a, w)), "repeatable"
-    _lib.lib.mmdp_set_gemm_pair(1)
 
 
 def test_gemm_strided_views():
@@ -114,8 +112,8 @@ def test_gemm_rejects_bad_arguments():
 
 @pytest.fixture(params=[6, 7])
 def attn_version(request):
-    """Both attention kernel generations (csrc/attention6.cu: the default; attention7.cu: one CTA per SM with two query tiles,
-    opt-in through MMDP_ATTN_VERSION / mmdp_set_option) run the same tests."""
+    """Both attention kernel generations of csrc/attention.cu (6: 128-key blocks, the default; 7: 64-key blocks, opt-in through
+    MMDP_ATTN_VERSION / mmdp_set_option) run the same tests."""
     from mmada_parallel_b200 import _lib
     _lib.check(_lib.lib.mmdp_set_option(b"attn_version", request.param))
     yield request.param
@@ -179,8 +177,8 @@ def test_qkv_rope_and_attention(B, L, H, attn_version):
 
 def test_attention_lazy_rescale(attn_version):
     """The attention kernel against the fp32 reference, on random scores and on
-    scores whose magnitude grows along the KV axis, so that the running row max jumps by far more than the lazy-rescale
-    threshold (2^8) in many KV blocks - the path that rescales the TMEM-resident O accumulator."""
+    scores whose magnitude grows along the KV axis, so that the running row max jumps by far more than 2^8 in many KV
+    blocks - the path that rescales the register-resident O accumulator."""
     from mmada_parallel_b200 import _lib
     scale = 1.0 / math.sqrt(128.0)
     version = attn_version
@@ -207,8 +205,8 @@ def test_attention_lazy_rescale(attn_version):
 
 def test_attention_bitwise_repeatable(attn_version):
     """The same attention launch repeated many times at the full sequence length must be bitwise identical. (A parity wait
-    that could return two mbarrier phases early made v6 read O before the last PV MMAs retired - rare, timing dependent,
-    a few query rows per launch; this is the stress that exposes such races.) Two co-resident CTAs per SM, B=2."""
+    that returns an mbarrier phase early lets a warpgroup read a K / V^T stage before its TMA load landed, or the producer
+    overwrite one still in use - rare, timing dependent; this is the stress that exposes such races.) B=2."""
     from mmada_parallel_b200 import _lib
     B, L, H = 2, 2414, 16
     d, M, Lpad = H * 128, 2 * 2414, 2416
@@ -247,7 +245,7 @@ def test_rmsnorm_embed_lfq():
 
 
 def test_attention_full_length_relative_error(attn_version):
-    """BASELINE sequence length, 32 heads (608 CTAs: two full waves + the KV-split partial wave and its combine pass) against
+    """BASELINE sequence length, 32 heads (608 query tiles: four full waves of 132 SMs + a partial one) against
     the fp32 reference with the relative bound of assert_attention_close; also checks the split and unsplit tails agree."""
     from mmada_parallel_b200 import _lib
     B, L, H = 1, 2414, 32
@@ -302,15 +300,13 @@ def test_gemm_splitk_tail_matches_unsplit(epi):
     torch.manual_seed(12)
     fn = run()
     try:
-        _lib.lib.mmdp_set_gemm_pair(0)  # the 1-CTA kernel (default for M <= 256; the pair kernel has no split-K tail)
-        _lib.lib.mmdp_set_gemm_splitk(0)
+        _lib.lib.mmdp_set_gemm_splitk(0)  # (the default 1-CTA kernel; the pair kernel has no split-K tail)
         ref = fn()
         _lib.lib.mmdp_set_gemm_splitk(3)  # split whenever a partial last wave exists
         got = fn()
         again = fn()
     finally:
         _lib.lib.mmdp_set_gemm_splitk(2)
-        _lib.lib.mmdp_set_gemm_pair(1)
     assert torch.equal(got, again), "split-K tail must be deterministic"
     diff = (got - ref).abs()
     scale = ref.abs().max().item()
@@ -320,8 +316,8 @@ def test_gemm_splitk_tail_matches_unsplit(epi):
 
 @pytest.mark.parametrize("M,N,K", [(777, 1000, 520), (2414, 4096, 1024), (300, 512, 768)])
 def test_gemm_pair_kernel_bit_identical_to_single(M, N, K):
-    """The CTA-pair (cta_group::2) kernel - the default for M > 256 - accumulates K in the same order as the 1-CTA kernel
-    without its split-K tail: plain, residual and SwiGLU epilogues must agree bit for bit."""
+    """The CTA-pair kernel (a 2-CTA cluster sharing the W tile by TMA multicast, opt-in through MMDP_GEMM_PAIR) accumulates K
+    in the same order as the 1-CTA kernel without its split-K tail: plain, residual and SwiGLU epilogues must agree bit for bit."""
     from mmada_parallel_b200 import _lib
     torch.manual_seed(M + K)
     a = bf(torch.randn(M, K, device="cuda") * 0.5)
@@ -340,58 +336,4 @@ def test_gemm_pair_kernel_bit_identical_to_single(M, N, K):
             assert torch.equal(got, ref), epi
     finally:
         _lib.lib.mmdp_set_gemm_splitk(2)
-        _lib.lib.mmdp_set_gemm_pair(1)
-
-
-@pytest.mark.parametrize("epi,M,N,K", [("qkv", 2414, 12288, 4096), ("plain", 2414, 23040, 448), ("resid", 2300, 4864, 576)])
-def test_gemm_pair_tail_nsplit_bit_identical(epi, M, N, K):
-    """Tail N-split of the CTA-pair kernel (gemm2.cu): the tiles of a partial last wave are cut into two half-width units. Every
-    output element still sees the same K loop, so the result must equal the unsplit kernel's bit for bit (QKV + rotary at the
-    bench shape: 480 tiles = 6 waves of 74 + 36 tiles -> 72 half units; plain 900 tiles -> tail 12; residual 171 -> tail 23)."""
-    from mmada_parallel_b200 import _lib
-    from mmada_parallel_b200.model import rope_tables
-    torch.manual_seed(M + N + K)
-    a = bf(torch.randn(M, K, device="cuda") * 0.5)
-    w = bf(torch.randn(N, K, device="cuda") / math.sqrt(K))
-    if epi == "qkv":
-        H = N // 3 // 128
-        cos, sin = (t.cuda() for t in rope_tables(128, 500000.0, M))
-        fn = lambda: torch.cat([t.reshape(-1).float() for t in _lib.qkv_rope(a, w, H, M, cos, sin)])
-    elif epi == "plain":
-        fn = lambda: _lib.gemm_bf16(a, w, _lib.EPI_PLAIN).float()
-    else:
-        r = bf(torch.randn(M, N, device="cuda"))
-        fn = lambda: _lib.gemm_bf16(a, w, _lib.EPI_RESID, resid=r).float()
-    try:
-        _lib.check(_lib.lib.mmdp_set_option(b"gemm_nsplit_tail", 0))
-        ref = fn()
-        _lib.check(_lib.lib.mmdp_set_option(b"gemm_nsplit_tail", 1))
-        got = fn()
-        again = fn()
-    finally:
-        _lib.check(_lib.lib.mmdp_set_option(b"gemm_nsplit_tail", 1))
-    assert torch.equal(got, ref), epi
-    assert torch.equal(got, again)
-
-
-@pytest.mark.parametrize("M,N,K", [(2414, 24576, 4096), (2414, 24576, 320), (1100, 5120, 576), (2432, 6144, 448), (2305, 24576, 256), (2500, 24576, 256)])
-def test_gemm_pair_swiglu_half_m_units_bit_identical(M, N, K):
-    """SwiGLU GEMM of the CTA-pair kernel with the last m-block (M % 256 <= 128) computed as 128-row half-M units (cta_group::2 MMAs
-    with M = 128, 64 rows per CTA, W rows re-ordered so that a TMEM lane half holds [64 gate | 64 up] of the same outputs): the same
-    K loop per element, so the result must equal the 256-row-tile schedule bit for bit. (2500 rows: 196 valid rows in the last
-    block, the path is not taken; 2305: a single valid row in it.)"""
-    from mmada_parallel_b200 import _lib
-    torch.manual_seed(M + N + K)
-    a = bf(torch.randn(M, K, device="cuda") * 0.5)
-    w = bf(torch.randn(N, K, device="cuda") / math.sqrt(K))
-    try:
-        _lib.check(_lib.lib.mmdp_set_option(b"gemm_mtail", 0))
-        ref = _lib.gemm_bf16(a, w, _lib.EPI_SWIGLU)
-        _lib.check(_lib.lib.mmdp_set_option(b"gemm_mtail", 1))
-        got = _lib.gemm_bf16(a, w, _lib.EPI_SWIGLU)
-        again = _lib.gemm_bf16(a, w, _lib.EPI_SWIGLU)
-    finally:
-        _lib.check(_lib.lib.mmdp_set_option(b"gemm_mtail", 1))
-    assert not torch.isnan(got.float()).any()
-    assert torch.equal(got, ref), f"max |d| {(got.float() - ref.float()).abs().max().item()}"
-    assert torch.equal(got, again)
+        _lib.lib.mmdp_set_gemm_pair(0)

@@ -1,8 +1,8 @@
-"""MAGVITv2.decode_code on the B200 (TF32 tcgen05 convolutions) against the golden images produced by the REAL
+"""MAGVITv2.decode_code on the H100 (TF32 wgmma convolutions) against the golden images produced by the REAL
 reference decoder (fp32, CPU; oracle pinned bit-exact in oracle/make_golden_magvit.py).
 Floating-point tolerance (stated): TF32 products (10-bit mantissa) through ~35 convolutions with GroupNorm in between;
-per-pixel |err| <= 0.02 and mean |err| <= 0.003 on images with std ~0.55, |max| ~3.4 (measured on the B200: max 0.0078,
-mean 0.0013 - well inside one 8-bit pixel step, 1/127.5 = 0.0078 after the caller's (x+1)/2 mapping).
+per-pixel |err| <= 0.02 and mean |err| <= 0.003 on images with std ~0.55, |max| ~3.4 (the test prints the measured errors;
+one 8-bit pixel step is 1/127.5 = 0.0078 after the caller's (x+1)/2 mapping).
 Deviation from torch's defaults, stated: every contraction of the decoder runs with TF32 products, including the two
 matmuls of the mid-block AttnBlock; torch.backends.cuda.matmul.allow_tf32 defaults to False (fp32 matmul) while cuDNN
 convolutions default to TF32, so the reference on a GPU would run those two matmuls in fp32 - 2 of ~60 contractions,

@@ -1,4 +1,4 @@
-"""Whole-path parity on the B200: native forward vs the reference's logits (golden), and the generation loops vs the
+"""Whole-path parity on the H100: native forward vs the reference's logits (golden), and the generation loops vs the
 oracle running on the SAME logits (bit-exact integer decisions), plus the real-reference golden trajectories."""
 import contextlib
 import io
@@ -62,7 +62,7 @@ def _args(lay):
 
 
 def test_generate_ti2ti_lockstep_with_oracle():
-    """Product loop (CUDA kernels) == oracle loop (CPU) when both see the B200's logits: every token id equal."""
+    """Product loop (CUDA kernels) == oracle loop (CPU) when both see the H100's logits: every token id equal."""
     from mmada_parallel_b200.generators.parallel_generator import generate_ti2ti
     t = load_golden("trajectory_a_tiny.pt")
     model, cfg, _ = tiny_gpu_model(t["meta"])
@@ -266,7 +266,7 @@ def _device_view_bf16(ptr_value, numel):
 
 def test_full_size_block_and_head_vs_oracle():
     """BASELINE shapes against the ORACLE (not against itself): one LLaDA block at d=4096 / ff=12288 / 32 heads / L=2414 plus
-    the restricted LM head (256 text rows x 134 656 columns, 1024 image rows x the 8192-column codebook window), B200 vs
+    the restricted LM head (256 text rows x 134 656 columns, 1024 image rows x the 8192-column codebook window), H100 vs
     oracle.llada on the box's CPU with the same bf16 weights. This is the production tile schedule: 19 m-tiles, the split-K
     tails of the GEMMs, 608 attention CTAs with the KV-split partial wave. Bound: 4 bf16 ulp of the tensor's scale (same as
     the tiny-model logit test), and the mean error far below one ulp."""
@@ -417,7 +417,7 @@ class _RecordingDecoder:
 
 
 def test_generate_ti2ti_stepwise_lockstep_with_oracle():
-    """Preview loop (A/app.py:143-398, SURVEY 8f rank 2): product generator == oracle generator on the B200's logits -
+    """Preview loop (A/app.py:143-398, SURVEY 8f rank 2): product generator == oracle generator on the H100's logits -
     every yielded (step, text, status), the ids handed to the decoder, and the greyed-out (re-masked) cells."""
     from mmada_parallel_b200.generators.stepwise import generate_ti2ti_stepwise
     t = load_golden("trajectory_stepwise_tiny.pt")
@@ -479,7 +479,7 @@ def test_decode_vq_to_image_native_decoder():
 
 
 def test_mmu_generate_lockstep_with_oracle():
-    """MMadaModelLM.mmu_generate (M/models/modeling_mmada.py:619-691, SURVEY 8f rank 3): product == oracle on the B200's
+    """MMadaModelLM.mmu_generate (M/models/modeling_mmada.py:619-691, SURVEY 8f rank 3): product == oracle on the H100's
     logits, every id of every batch row; plus the golden outputs of the real reference as a reported agreement."""
     from mmada_parallel_b200.mmada import MMadaModelLM
     t = load_golden("trajectory_mmu_tiny.pt")

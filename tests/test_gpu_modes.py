@@ -1,4 +1,4 @@
-"""Adjacent generation modes of SURVEY.md section 8f rank 3 on the B200, each in lock-step with the oracle running on the
+"""Adjacent generation modes of SURVEY.md section 8f rank 3 on the H100, each in lock-step with the oracle running on the
 SAME (GPU-computed) logits and the same replayed noise - integer outputs must be equal at every step:
   A  generate_image        (generators/image_generation_generator.py:15-251, MaskGit text-to-image)
   M  t2i_generate          (models/modeling_mmada.py:265-359)

@@ -15,7 +15,7 @@ pytestmark = pytest.mark.gpu
 def test_tensor_parallel_matches_single_gpu():
     n = torch.cuda.device_count()
     if n < 2:
-        pytest.skip("needs >= 2 GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs >= 2 GPUs")
     tp = 2
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={tp}", "--master-addr", "127.0.0.1",
            "--master-port", "29631", os.path.join(ROOT, "tests", "_tp_worker.py")]

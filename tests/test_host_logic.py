@@ -106,7 +106,7 @@ def test_tensor_parallel_sharding_math():
 
 def test_gemm_tile_order_is_a_bijection(tmp_path):
     """The grouped-M tile order of the persistent GEMM (csrc/gemm_epilogue.cuh::gemm_tile_coords) visits every tile exactly
-    once for every group size, and halves the m-span of a 148-tile wave at 57 m-tiles. Host-only: the function is
+    once for every group size, and halves the m-span of a 132-tile wave at 57 m-tiles. Host-only: the function is
     __host__ __device__, the check is compiled with nvcc and runs on the CPU (tests/host/tile_order.cu)."""
     import shutil
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
@@ -195,10 +195,7 @@ def test_bench_workload_shapes_and_counts():
 def test_tensor_parallel_chunk_split_and_half_m_unit_schedule():
     """chunk_split (row chunks of the pipelined tensor-parallel forward): one chunk below 1024 rows, else two chunks that cover
     [0, M), the first a multiple of 256 rows, chunk 1 never above half the rows (its buffers are sized for that) and every rank owns at
-    least one row of each chunk up to TP=8. And the host restatement of the half-M unit placement of the SwiGLU GEMM
-    (csrc/gemm2.cu: the half unit of n-tile g sits at position (g / period) % num_m, period = clusters / gcd(num_m, clusters)): with
-    unit % clusters as the unit -> cluster map every cluster gets its share of the half units."""
-    from math import gcd
+    least one row of each chunk up to TP=8."""
     from mmada_parallel_b200.tensor_parallel import chunk_split, row_partition
     assert chunk_split(1023) == [1023] and chunk_split(60) == [60]
     for M in (1024, 1500, 2341, 2414, 4682, 4828, 4096):
@@ -207,18 +204,3 @@ def test_tensor_parallel_chunk_split_and_half_m_unit_schedule():
         for rows in parts:
             for tp in (2, 4, 8):
                 assert row_partition(rows, tp, tp - 1)[1] >= 1
-    clusters = 74
-    for M, N in ((2414, 24576), (4682, 24576), (2414, 3072 * 2)):
-        num_m, num_n = (M + 255) // 256, N // 256
-        period = clusters // gcd(num_m, clusters)
-        load = [0.0] * clusters
-        halves = [0] * clusters
-        for u in range(num_m * num_n):
-            g, o = divmod(u, num_m)
-            half = o == (g // period) % num_m
-            load[u % clusters] += 0.5 if half else 1.0
-            halves[u % clusters] += half
-        assert sum(halves) == num_n
-        if num_n >= clusters:       # enough half units for everybody: nobody is left with a full extra tile
-            assert min(halves) >= 1
-            assert max(load) <= (num_m * num_n - 0.5 * num_n) / clusters + 0.75

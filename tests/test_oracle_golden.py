@@ -225,7 +225,7 @@ def test_variant_m_modes_match_reference_golden(tiny):
 
 def test_separated_model_trajectories_match_reference_golden():
     """The "well-separated" tiny model (oracle/make_golden_separated.py): the oracle reproduces the REAL reference's per-step ids
-    on all three configurations (greedy / bench-like / both CFGs + text Gumbel) - the fixture the B200 path must match bit for
+    on all three configurations (greedy / bench-like / both CFGs + text Gumbel) - the fixture the H100 path must match bit for
     bit in tests/test_gpu_model.py::test_trajectory_bit_equal_to_reference_on_separated_model."""
     from oracle.make_golden_separated import separated_weights, trajectory
     t = load_golden("trajectory_a_separated.pt")
