@@ -142,6 +142,24 @@ MMDP_API int mmdp_tp_forward(const mmdp_tp_ctx* c, const int64_t* ids, int B, in
 MMDP_API int mmdp_gemm_bf16(int epilogue, const uint16_t* A, int lda, const uint16_t* W, int ldw, int M, int N, int K,
                    uint16_t* C, int ldc, const uint16_t* R, int ldr, void* stream);
 
+/* ---- FP8 (e4m3) linears (csrc/fp8.cu; the opt-in precision of mmdp_model_create_ex) ---------------------------------
+ * Quantiser, one definition for weights and activations: for a row group g of `group` elements,
+ *   s = amax(|x|) / 448 in fp32 (IEEE division; s = 1 for an all-zero group),   q = e4m3(x / s)  (IEEE division, round to
+ *   nearest even, saturating; the bytes equal torch's x.float().div(s).to(float8_e4m3fn)).
+ * mmdp_quantize_fp8: x bf16 [rows, K] (row stride ldx) -> q e4m3 [rows, K] (row stride ldq) and scales fp32 [K / group][rows]
+ *   (row index contiguous). group is a multiple of 128 that divides K: weights use group = K (one scale per row), activations
+ *   group = 128. ldx, ldq >= K and multiples of 4; x 8-byte, q 4-byte aligned.
+ * mmdp_gemm_fp8: C[M,N] = epilogue( sw[n] * sum_g sa[g][m] * sum_{k in g} A[m,k] W[n,k] ), fp32 accumulation; each 128-wide
+ *   k-block is summed by the tensor cores into a fresh fragment and then added to the fp32 accumulator with its activation
+ *   scale. A e4m3 [M, K] with scales sa [K/128][M] (from mmdp_quantize_fp8, group 128); W e4m3 [N, K] with row scales sw [N].
+ *   K % 128 == 0; lda, ldw multiples of 16. Epilogues PLAIN, RESID (as mmdp_gemm_bf16) and SWIGLU, for which the gate / up
+ *   rows of W are interleaved in 64-row blocks (the FP8 tile is 128 wide; the bf16 kernel interleaves 128-row blocks).
+ *   Every tile runs its whole K loop: the FP8 kernel has no split-K tail (MMDP_GEMM_SPLITK has no effect on it) and no
+ *   CTA-pair variant (MMDP_GEMM_PAIR has no effect on it). Results are deterministic. */
+MMDP_API int mmdp_quantize_fp8(const uint16_t* x, int ldx, int rows, int K, int group, uint8_t* q, int ldq, float* scales, void* stream);
+MMDP_API int mmdp_gemm_fp8(int epilogue, const uint8_t* A, int lda, const float* sa, const uint8_t* W, int ldw, const float* sw, int M,
+                           int N, int K, uint16_t* C, int ldc, const uint16_t* R, int ldr, void* stream);
+
 /* q/k/v projection + rotary embedding (modeling_llada.py:925-927, RotaryEmbedding :402-435).
  * Wqkv = [q_proj; k_proj; v_proj] rows ([3*d_model, d_model]); A = normed activations [B*L, d_model].
  * Outputs: q,k [B*L, d_model] with RoPE applied (fp32 math on the bf16-rounded projections, positions 0..L-1 per batch row);
@@ -276,6 +294,15 @@ typedef struct {
 } mmdp_model_config;
 
 MMDP_API int mmdp_model_create(const mmdp_model_config* cfg, mmdp_model** out);
+/* Precision of the four linears of every block (q/k/v_proj, attn_out, ff_proj/up_proj, ff_out). mmdp_model_create means BF16.
+ * FP8: those weights are quantised to e4m3 with one fp32 scale per output row in mmdp_model_set_weight (no bf16 copy is
+ * kept); every forward quantises their bf16 inputs (xn after attn_norm / ff_norm, the attention output, the SwiGLU output)
+ * in 1 x 128 groups and runs mmdp_gemm_fp8 with the same fused epilogues. The embedding, norms, RoPE, attention, residual
+ * adds, the SwiGLU rounding points, ln_f and the LM head stay bf16 as in a BF16 context. d_model and mlp_hidden are
+ * multiples of 128 (checked for both precisions). */
+#define MMDP_PRECISION_BF16 0
+#define MMDP_PRECISION_FP8 1
+MMDP_API int mmdp_model_create_ex(const mmdp_model_config* cfg, int precision, mmdp_model** out);
 MMDP_API void mmdp_model_destroy(mmdp_model* m);
 
 /* Copies (and packs) one tensor of the HF state dict into the model-owned device buffers. `src` may be a device or

@@ -16,6 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libmmdp.so")
 
 EPI_PLAIN, EPI_RESID, EPI_SWIGLU, EPI_F32 = 0, 1, 3, 4
+PRECISION_BF16, PRECISION_FP8 = 0, 1
 
 
 class MmdpError(RuntimeError):
@@ -91,6 +92,8 @@ SIGNATURES = {
     "mmdp_gemm_f32_scatter": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),
     "mmdp_tp_reduce_norm": (_i, [_vp, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _i, _f, C.c_uint32, _vp, _vp]),
     "mmdp_gemm_bf16": (_i, [_i, _vp, _i, _vp, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp]),
+    "mmdp_quantize_fp8": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _vp, _vp]),
+    "mmdp_gemm_fp8": (_i, [_i, _vp, _i, _vp, _vp, _i, _vp, _i, _i, _i, _vp, _i, _vp, _i, _vp]),
     "mmdp_qkv_rope": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mmdp_qkv_rope_tp": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mmdp_resid_add_f32": (_i, [_vp, _i, _vp, _i, _i, _i, _vp]),
@@ -114,6 +117,7 @@ SIGNATURES = {
     "mmdp_vqenc_create": (_i, [C.POINTER(VqDecConfig), C.POINTER(_vp)]),
     "mmdp_vqenc_encode": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
     "mmdp_model_create": (_i, [C.POINTER(ModelConfig), C.POINTER(_vp)]),
+    "mmdp_model_create_ex": (_i, [C.POINTER(ModelConfig), _i, C.POINTER(_vp)]),
     "mmdp_model_destroy": (None, [_vp]),
     "mmdp_model_set_weight": (_i, [_vp, C.c_char_p, _vp, _i64, _i64, _vp]),
     "mmdp_model_set_rope": (_i, [_vp, _vp, _vp, _i, _vp]),
@@ -177,6 +181,36 @@ def gemm_bf16(a: torch.Tensor, w: torch.Tensor, epilogue: int = EPI_PLAIN, resid
         out = torch.empty((M, n_out), dtype=torch.bfloat16, device=a.device)
     check(lib.mmdp_gemm_bf16(epilogue, ptr(a), a.stride(0), ptr(w), w.stride(0), M, N, K, ptr(out), out.stride(0),
                              ptr(resid), resid.stride(0) if resid is not None else 0, stream_ptr()))
+    return out
+
+
+def quantize_fp8(x: torch.Tensor, group: int = 128):
+    """e4m3 quantisation of a bf16 [rows, K] tensor (row stride may exceed K) in row groups of `group` elements.
+    Returns (q float8_e4m3fn [rows, K], scales fp32 [K // group, rows])."""
+    require_cuda(x)
+    assert x.dtype == torch.bfloat16 and x.dim() == 2 and x.stride(1) == 1
+    rows, K = x.shape
+    q = torch.empty((rows, K), dtype=torch.float8_e4m3fn, device=x.device)
+    s = torch.empty((K // group, rows), dtype=torch.float32, device=x.device)
+    check(lib.mmdp_quantize_fp8(ptr(x), x.stride(0), rows, K, group, ptr(q), K, ptr(s), stream_ptr()))
+    return q, s
+
+
+def gemm_fp8(qa: torch.Tensor, sa: torch.Tensor, qw: torch.Tensor, sw: torch.Tensor, epilogue: int = EPI_PLAIN,
+             resid: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """C = epilogue(sw[n] * sum_g sa[g, m] * (qa[m, g] . qw[n, g])): qa [M, K] e4m3 with scales sa [K/128, M], qw [N, K] e4m3
+    with row scales sw [N]. For EPI_SWIGLU the gate / up rows of qw (and sw) are interleaved in 64-row blocks."""
+    require_cuda(qa, sa, qw, sw, resid, out)
+    assert qa.dtype == torch.float8_e4m3fn and qw.dtype == torch.float8_e4m3fn
+    assert sa.dtype == torch.float32 and sw.dtype == torch.float32 and sa.is_contiguous() and sw.is_contiguous()
+    M, K = qa.shape
+    N = qw.shape[0]
+    assert tuple(sa.shape) == (K // 128, M) and tuple(sw.shape) == (N,)
+    n_out = N // 2 if epilogue == EPI_SWIGLU else N
+    if out is None:
+        out = torch.empty((M, n_out), dtype=torch.bfloat16, device=qa.device)
+    check(lib.mmdp_gemm_fp8(epilogue, ptr(qa), qa.stride(0), ptr(sa), ptr(qw), qw.stride(0), ptr(sw), M, N, K, ptr(out),
+                            out.stride(0), ptr(resid), resid.stride(0) if resid is not None else 0, stream_ptr()))
     return out
 
 

@@ -43,6 +43,10 @@ struct LayerWeights {
     bf16* w2;         // [d, ff]
     bf16* attn_norm;  // [d]
     bf16* ff_norm;    // [d]
+    // FP8 context: the four linears as e4m3 (same row order, except that W13 interleaves 64-row blocks, the gate / up halves
+    // of the FP8 GEMM's 128-wide tile) with one fp32 scale per row; the bf16 pointers above are then null
+    uint8_t *wqkv8 = nullptr, *wo8 = nullptr, *w13_8 = nullptr, *w2_8 = nullptr;
+    float *sqkv = nullptr, *so = nullptr, *s13 = nullptr, *s2 = nullptr;
 };
 
 struct mmdp_model {
@@ -59,6 +63,9 @@ struct mmdp_model {
     bf16 *x = nullptr, *xn = nullptr, *q = nullptr, *k = nullptr, *vt = nullptr, *att = nullptr, *h = nullptr, *xr = nullptr;
     int* err_flag = nullptr;  // device: bit 0 = token id out of range, bit 1 = logits row index out of range
     int vt_B = 0, vt_Lpad = 0, vt_L = 0;  // layout / length the vt buffer was last zeroed for
+    int precision = MMDP_PRECISION_BF16;
+    uint8_t* a8 = nullptr;  // FP8: the quantised input of the current linear, [M, K] e4m3
+    float* as = nullptr;    // FP8: its scales, [K / 128][M]
     std::vector<void*> allocs;
 };
 
@@ -80,6 +87,17 @@ MMDP_API int mmdp_gemm_bf16(int epilogue, const uint16_t* A, int lda, const uint
         return set_error("mmdp_gemm_bf16: unknown epilogue %d", epilogue);
     return gemm_bf16(epilogue, (const bf16*)A, lda, (const bf16*)W, ldw, M, N, K, (bf16*)C, ldc, (const bf16*)R, ldr,
                      nullptr, (cudaStream_t)stream);
+}
+
+MMDP_API int mmdp_quantize_fp8(const uint16_t* x, int ldx, int rows, int K, int group, uint8_t* q, int ldq, float* scales, void* stream) {
+    return quantize_fp8((const bf16*)x, ldx, rows, K, group, q, ldq, scales, (cudaStream_t)stream);
+}
+
+MMDP_API int mmdp_gemm_fp8(int epilogue, const uint8_t* A, int lda, const float* sa, const uint8_t* W, int ldw, const float* sw, int M,
+                           int N, int K, uint16_t* C, int ldc, const uint16_t* R, int ldr, void* stream) {
+    if (epilogue != MMDP_EPI_PLAIN && epilogue != MMDP_EPI_RESID && epilogue != MMDP_EPI_SWIGLU)
+        return set_error("mmdp_gemm_fp8: unsupported epilogue %d", epilogue);
+    return gemm_fp8(epilogue, A, lda, sa, W, ldw, sw, M, N, K, (bf16*)C, ldc, (const bf16*)R, ldr, nullptr, (cudaStream_t)stream);
 }
 
 MMDP_API int mmdp_qkv_rope(const uint16_t* A, int lda, const uint16_t* Wqkv, int M, int d_model, int n_heads, int L, int Lpad,
@@ -327,9 +345,16 @@ MMDP_API int mmdp_set_option(const char* key, int value) { return key ? set_opt(
 // model context
 // ------------------------------------------------------------------------------------------------
 MMDP_API int mmdp_model_create(const mmdp_model_config* c, mmdp_model** out) {
+    return mmdp_model_create_ex(c, MMDP_PRECISION_BF16, out);
+}
+
+MMDP_API int mmdp_model_create_ex(const mmdp_model_config* c, int precision, mmdp_model** out) {
     if (!c || !out) return set_error("mmdp_model_create: null argument");
+    if (precision != MMDP_PRECISION_BF16 && precision != MMDP_PRECISION_FP8)
+        return set_error("mmdp_model_create: unknown precision %d", precision);
     if (c->d_model != c->n_heads * 128) return set_error("mmdp_model_create: head_dim must be 128");
     if (c->d_model % 256) return set_error("mmdp_model_create: d_model must be a multiple of 256");
+    // (both also make every K of the FP8 linears a multiple of its 128-wide activation scale group)
     if (c->mlp_hidden % 128) return set_error("mmdp_model_create: mlp_hidden must be a multiple of 128");
     if (c->vocab_size % 8) return set_error("mmdp_model_create: vocab_size must be a multiple of 8");
     if (c->n_layers <= 0 || c->max_seq_len <= 0 || c->max_batch <= 0) return set_error("mmdp_model_create: bad sizes");
@@ -338,14 +363,26 @@ MMDP_API int mmdp_model_create(const mmdp_model_config* c, mmdp_model** out) {
         return set_error("mmdp_model_create: no CUDA device (this library has no CPU fallback)");
     mmdp_model* m = new mmdp_model();
     m->cfg = *c;
+    m->precision = precision;
     const size_t d = c->d_model, ff = c->mlp_hidden, V = c->vocab_size;
     m->layers.resize(c->n_layers);
     int rc = 0;
     for (auto& l : m->layers) {
-        rc |= dev_alloc(m, (void**)&l.wqkv, 3 * d * d * 2);
-        rc |= dev_alloc(m, (void**)&l.wo, d * d * 2);
-        rc |= dev_alloc(m, (void**)&l.w13, 2 * ff * d * 2);
-        rc |= dev_alloc(m, (void**)&l.w2, d * ff * 2);
+        if (precision == MMDP_PRECISION_FP8) {
+            rc |= dev_alloc(m, (void**)&l.wqkv8, 3 * d * d);
+            rc |= dev_alloc(m, (void**)&l.wo8, d * d);
+            rc |= dev_alloc(m, (void**)&l.w13_8, 2 * ff * d);
+            rc |= dev_alloc(m, (void**)&l.w2_8, d * ff);
+            rc |= dev_alloc(m, (void**)&l.sqkv, 3 * d * 4);
+            rc |= dev_alloc(m, (void**)&l.so, d * 4);
+            rc |= dev_alloc(m, (void**)&l.s13, 2 * ff * 4);
+            rc |= dev_alloc(m, (void**)&l.s2, d * 4);
+        } else {
+            rc |= dev_alloc(m, (void**)&l.wqkv, 3 * d * d * 2);
+            rc |= dev_alloc(m, (void**)&l.wo, d * d * 2);
+            rc |= dev_alloc(m, (void**)&l.w13, 2 * ff * d * 2);
+            rc |= dev_alloc(m, (void**)&l.w2, d * ff * 2);
+        }
         rc |= dev_alloc(m, (void**)&l.attn_norm, d * 2);
         rc |= dev_alloc(m, (void**)&l.ff_norm, d * 2);
     }
@@ -362,6 +399,10 @@ MMDP_API int mmdp_model_create(const mmdp_model_config* c, mmdp_model** out) {
     rc |= dev_alloc(m, (void**)&m->att, Mm * d * 2);
     rc |= dev_alloc(m, (void**)&m->xr, Mm * d * 2);
     rc |= dev_alloc(m, (void**)&m->h, Mm * ff * 2);
+    if (precision == MMDP_PRECISION_FP8) {  // the widest linear input is h: K = mlp_hidden
+        rc |= dev_alloc(m, (void**)&m->a8, Mm * ff);
+        rc |= dev_alloc(m, (void**)&m->as, Mm * (ff / 128) * 4);
+    }
     rc |= dev_alloc(m, (void**)&m->vt, (size_t)c->max_batch * d * m->Lpad_max * 2);
     rc |= dev_alloc(m, (void**)&m->cos_tab, (size_t)c->max_seq_len * 64 * 4);
     rc |= dev_alloc(m, (void**)&m->sin_tab, (size_t)c->max_seq_len * 64 * 4);
@@ -386,6 +427,39 @@ static int copy_rows(void* dst, const void* src, size_t bytes, cudaStream_t s) {
     return 0;
 }
 
+// FP8 context: one linear of a block [rows, cols] (bf16, device or host) -> e4m3 with one scale per row (group = cols), written
+// into the packed layer matrices. The bf16 source is staged on the device and never kept.
+static int set_weight_fp8(LayerWeights& l, const char* sub, const void* src, int64_t rows, int64_t cols, cudaStream_t s) {
+    const size_t n = (size_t)rows * cols;
+    const bool w13 = !strcmp(sub, "up_proj") || !strcmp(sub, "ff_proj");
+    bf16* stage = nullptr;
+    uint8_t* q = nullptr;
+    float* sc = nullptr;
+    MMDP_CUDA(cudaMallocAsync((void**)&stage, n * 2 + (w13 ? n + rows * 4 : 0), s));
+    int rc = copy_rows(stage, src, n * 2, s);
+    if (!strcmp(sub, "attn_out")) { q = l.wo8; sc = l.so; }
+    else if (!strcmp(sub, "ff_out")) { q = l.w2_8; sc = l.s2; }
+    else if (!w13) {
+        const int which = sub[0] == 'q' ? 0 : (sub[0] == 'k' ? 1 : 2);
+        q = l.wqkv8 + (size_t)which * n;
+        sc = l.sqkv + (size_t)which * rows;
+    } else {  // quantised next to the stage, then interleaved: source block t of 64 rows -> destination block 2t + up
+        q = reinterpret_cast<uint8_t*>(stage + n);
+        sc = reinterpret_cast<float*>(q + n);
+    }
+    if (!rc) rc = quantize_fp8(stage, (int)cols, (int)rows, (int)cols, (int)cols, q, (int)cols, sc, s);
+    if (!rc && w13) {
+        const size_t up = !strcmp(sub, "up_proj") ? 1 : 0;
+        const cudaError_t e1 = cudaMemcpy2DAsync(l.w13_8 + up * 64 * cols, 128 * cols, q, 64 * cols, 64 * cols, rows / 64,
+                                                 cudaMemcpyDeviceToDevice, s);
+        const cudaError_t e2 = cudaMemcpy2DAsync(l.s13 + up * 64, 128 * 4, sc, 64 * 4, 64 * 4, rows / 64, cudaMemcpyDeviceToDevice, s);
+        if (e1 != cudaSuccess || e2 != cudaSuccess) rc = set_error("mmdp_model_set_weight: packing W13 failed: %s", cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
+    }
+    const cudaError_t ef = cudaFreeAsync(stage, s);
+    if (!rc && ef != cudaSuccess) rc = set_error("mmdp_model_set_weight: cudaFreeAsync failed: %s", cudaGetErrorString(ef));
+    return rc;
+}
+
 MMDP_API int mmdp_model_set_weight(mmdp_model* m, const char* name, const void* src, int64_t rows, int64_t cols, void* stream) {
     if (!m || !name || !src) return set_error("mmdp_model_set_weight: null argument");
     cudaStream_t s = (cudaStream_t)stream;
@@ -405,6 +479,16 @@ MMDP_API int mmdp_model_set_weight(mmdp_model* m, const char* name, const void* 
     if (sscanf(name, "blocks.%d.%63s", &li, sub) != 2 || li < 0 || li >= m->cfg.n_layers)
         return set_error("mmdp_model_set_weight: unknown tensor name '%s'", name);
     LayerWeights& l = m->layers[li];
+    if (m->precision == MMDP_PRECISION_FP8) {
+        const bool qkv = !strcmp(sub, "q_proj") || !strcmp(sub, "k_proj") || !strcmp(sub, "v_proj");
+        const bool w13 = !strcmp(sub, "ff_proj") || !strcmp(sub, "up_proj");
+        const bool wo = !strcmp(sub, "attn_out"), w2 = !strcmp(sub, "ff_out");
+        if (qkv || w13 || wo || w2) {
+            const int64_t r = w13 ? ff : d, k = w2 ? ff : d;
+            if (expect(r, k)) return -1;
+            return set_weight_fp8(l, sub, src, r, k, s);
+        }
+    }
     if (!strcmp(sub, "q_proj") || !strcmp(sub, "k_proj") || !strcmp(sub, "v_proj")) {
         if (expect(d, d)) return -1;
         const int which = sub[0] == 'q' ? 0 : (sub[0] == 'k' ? 1 : 2);
@@ -448,6 +532,24 @@ MMDP_API int mmdp_model_error_flags(mmdp_model* m, int32_t* flags_host, void* st
     return 0;
 }
 
+// One of the four linears of block `l` (which: 0 = Wqkv, 1 = Wo, 2 = W13, 3 = W2) in the context's precision. FP8: the bf16
+// input A is quantised into the context's e4m3 workspace (1 x 128 groups), then the e4m3 GEMM applies the same epilogue.
+enum { LIN_QKV = 0, LIN_O = 1, LIN_13 = 2, LIN_2 = 3 };
+static int block_linear(mmdp_model* m, const LayerWeights& l, int which, int epi, const bf16* A, int lda, int M, bf16* C, int ldc,
+                        const bf16* R, int ldr, const QkvRopeArgs* qa, cudaStream_t s) {
+    const int d = m->cfg.d_model, ff = m->cfg.mlp_hidden;
+    const int N = which == LIN_QKV ? 3 * d : (which == LIN_13 ? 2 * ff : d);
+    const int K = which == LIN_2 ? ff : d;
+    if (m->precision == MMDP_PRECISION_BF16) {
+        const bf16* W = which == LIN_QKV ? l.wqkv : (which == LIN_O ? l.wo : (which == LIN_13 ? l.w13 : l.w2));
+        return gemm_bf16(epi, A, lda, W, K, M, N, K, C, ldc, R, ldr, qa, s);
+    }
+    const uint8_t* W = which == LIN_QKV ? l.wqkv8 : (which == LIN_O ? l.wo8 : (which == LIN_13 ? l.w13_8 : l.w2_8));
+    const float* sw = which == LIN_QKV ? l.sqkv : (which == LIN_O ? l.so : (which == LIN_13 ? l.s13 : l.s2));
+    if (quantize_fp8(A, lda, M, K, 128, m->a8, K, m->as, s)) return -1;
+    return gemm_fp8(epi, m->a8, K, m->as, W, K, sw, M, N, K, C, ldc, R, ldr, qa, s);
+}
+
 static int model_forward(mmdp_model* m, const int64_t* ids, int B, int L, uint16_t* full_logits, const int32_t* rows_a,
                          int n_a, uint16_t* out_a, const int32_t* rows_b, int n_b, int col0_b, int ncols_b,
                          uint16_t* out_b, int row_lo, int row_hi, void* stream) {
@@ -482,23 +584,23 @@ static int model_forward(mmdp_model* m, const int64_t* ids, int B, int L, uint16
         const LayerWeights& l = m->layers[li];
         const bool win = window && li == c.n_layers - 1;
         if (rmsnorm(m->x, d, l.attn_norm, m->xn, d, M, d, c.rms_eps, s)) return -1;
-        if (gemm_bf16(EPI_QKVROPE, m->xn, d, l.wqkv, d, M, 3 * d, d, nullptr, 0, nullptr, 0, &qa, s)) return -1;
+        if (block_linear(m, l, LIN_QKV, EPI_QKVROPE, m->xn, d, M, nullptr, 0, nullptr, 0, &qa, s)) return -1;
         if (!win) {
             if (attention_fwd(m->q, m->k, m->vt, m->att, B, H, L, Lpad, scale, s)) return -1;
-            if (gemm_bf16(EPI_RESID, m->att, d, l.wo, d, M, d, d, m->x, d, m->x, d, nullptr, s)) return -1;
+            if (block_linear(m, l, LIN_O, EPI_RESID, m->att, d, M, m->x, d, m->x, d, nullptr, s)) return -1;
             if (rmsnorm(m->x, d, l.ff_norm, m->xn, d, M, d, c.rms_eps, s)) return -1;
-            if (gemm_bf16(EPI_SWIGLU, m->xn, d, l.w13, d, M, 2 * ff, d, m->h, ff, nullptr, 0, nullptr, s)) return -1;
-            if (gemm_bf16(EPI_RESID, m->h, ff, l.w2, ff, M, d, ff, m->x, d, m->x, d, nullptr, s)) return -1;
+            if (block_linear(m, l, LIN_13, EPI_SWIGLU, m->xn, d, M, m->h, ff, nullptr, 0, nullptr, s)) return -1;
+            if (block_linear(m, l, LIN_2, EPI_RESID, m->h, ff, M, m->x, d, m->x, d, nullptr, s)) return -1;
             continue;
         }
         const int Mw = row_hi - row_lo;
         for (int b = 0; b < B; ++b) {  // one row range per batch row (B = 1, or the CFG batch of variant M)
             const size_t r0 = (size_t)b * L + row_lo, o_d = r0 * d, o_ff = r0 * ff;
             if (attention_fwd(m->q + o_d, m->k + (size_t)b * L * d, m->vt + (size_t)b * H * 128 * Lpad, m->att + o_d, 1, H, L, Lpad, scale, s, Mw)) return -1;
-            if (gemm_bf16(EPI_RESID, m->att + o_d, d, l.wo, d, Mw, d, d, m->x + o_d, d, m->x + o_d, d, nullptr, s)) return -1;
+            if (block_linear(m, l, LIN_O, EPI_RESID, m->att + o_d, d, Mw, m->x + o_d, d, m->x + o_d, d, nullptr, s)) return -1;
             if (rmsnorm(m->x + o_d, d, l.ff_norm, m->xn + o_d, d, Mw, d, c.rms_eps, s)) return -1;
-            if (gemm_bf16(EPI_SWIGLU, m->xn + o_d, d, l.w13, d, Mw, 2 * ff, d, m->h + o_ff, ff, nullptr, 0, nullptr, s)) return -1;
-            if (gemm_bf16(EPI_RESID, m->h + o_ff, ff, l.w2, ff, Mw, d, ff, m->x + o_d, d, m->x + o_d, d, nullptr, s)) return -1;
+            if (block_linear(m, l, LIN_13, EPI_SWIGLU, m->xn + o_d, d, Mw, m->h + o_ff, ff, nullptr, 0, nullptr, s)) return -1;
+            if (block_linear(m, l, LIN_2, EPI_RESID, m->h + o_ff, ff, Mw, m->x + o_d, d, m->x + o_d, d, nullptr, s)) return -1;
         }
     }
     if (full_logits) {
@@ -565,12 +667,12 @@ MMDP_API int mmdp_model_forward_cached(mmdp_model* m, const int64_t* ids, int B,
         bf16* vc = (bf16*)vtcache + (size_t)li * vt_layer;
         QkvRopeArgs qa{m->q, kc, vc, m->cos_tab, m->sin_tab, L, Lpad, d, H, pos_map, pos_map ? Tq : 0};
         if (rmsnorm(m->x, d, l.attn_norm, m->xn, d, M, d, c.rms_eps, s)) return -1;
-        if (gemm_bf16(EPI_QKVROPE, m->xn, d, l.wqkv, d, M, 3 * d, d, nullptr, 0, nullptr, 0, &qa, s)) return -1;
+        if (block_linear(m, l, LIN_QKV, EPI_QKVROPE, m->xn, d, M, nullptr, 0, nullptr, 0, &qa, s)) return -1;
         if (attention_fwd(m->q, kc, vc, m->att, B, H, L, Lpad, scale, s, Tq)) return -1;
-        if (gemm_bf16(EPI_RESID, m->att, d, l.wo, d, M, d, d, m->x, d, m->x, d, nullptr, s)) return -1;
+        if (block_linear(m, l, LIN_O, EPI_RESID, m->att, d, M, m->x, d, m->x, d, nullptr, s)) return -1;
         if (rmsnorm(m->x, d, l.ff_norm, m->xn, d, M, d, c.rms_eps, s)) return -1;
-        if (gemm_bf16(EPI_SWIGLU, m->xn, d, l.w13, d, M, 2 * ff, d, m->h, ff, nullptr, 0, nullptr, s)) return -1;
-        if (gemm_bf16(EPI_RESID, m->h, ff, l.w2, ff, M, d, ff, m->x, d, m->x, d, nullptr, s)) return -1;
+        if (block_linear(m, l, LIN_13, EPI_SWIGLU, m->xn, d, M, m->h, ff, nullptr, 0, nullptr, s)) return -1;
+        if (block_linear(m, l, LIN_2, EPI_RESID, m->h, ff, M, m->x, d, m->x, d, nullptr, s)) return -1;
     }
     if (logits) {
         if (rmsnorm(m->x, d, m->ln_f, m->xn, d, M, d, c.rms_eps, s)) return -1;

@@ -421,6 +421,17 @@ static int launch_gemm_pair(const CUtensorMap& tmA, const CUtensorMap& tmBh, con
 int gemm_pair_mode() { return opt(OPT_GEMM_PAIR); }
 void set_gemm_pair_mode(int on) { set_opt("gemm_pair", (on == 2) ? 2 : (on ? 1 : 0)); }
 
+int gemm_group_m(int M) {
+    const int group_m_env = opt(OPT_GEMM_GROUP_M);
+    const int num_m = (M + BM - 1) / BM;
+    int g = 0;
+    if (num_m > 45) {
+        const int ngroups = (num_m + 39) / 40;
+        g = (num_m + ngroups - 1) / ngroups;
+    }
+    return group_m_env >= 0 ? group_m_env : g;
+}
+
 int gemm_bf16(int epi, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int ldw, int M, int N, int K,
               __nv_bfloat16* C, int ldc, const __nv_bfloat16* resid, int ldr, const QkvRopeArgs* qa,
               cudaStream_t stream, const GemmScatter* sc) {
@@ -474,16 +485,7 @@ int gemm_bf16(int epi, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, 
     // spans ~30 m-tiles x a few n-tiles instead of all m-tiles x 2-3 n-tiles, which keeps the wave's A rows in L2 while the
     // weights stream (M = 7242: 57 m-tiles, the B=3 batch of a caller that batches its CFG branches); below ~45 m-tiles
     // the plain order is kept (M = 2414). MMDP_GEMM_GROUP_M overrides: 0 = off, n > 0 = fixed group size.
-    const int group_m_env = opt(OPT_GEMM_GROUP_M);
-    {
-        const int num_m = (M + BM - 1) / BM;
-        int g = 0;
-        if (num_m > 45) {
-            const int ngroups = (num_m + 39) / 40;
-            g = (num_m + ngroups - 1) / ngroups;
-        }
-        p.group_m = group_m_env >= 0 ? group_m_env : g;
-    }
+    p.group_m = gemm_group_m(M);
     if (qa) {
         p.q = qa->q; p.k = qa->k; p.vt = qa->vt; p.cos_tab = qa->cos_tab; p.sin_tab = qa->sin_tab;
         p.L = qa->L; p.Lpad = qa->Lpad; p.d_model = qa->d_model; p.n_heads = qa->n_heads;

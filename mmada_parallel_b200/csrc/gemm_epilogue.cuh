@@ -1,5 +1,5 @@
-// Fused epilogues of the bf16 GEMM kernel (gemm.cu). One call handles one thread's wgmma fragment of a 128 x BN
-// accumulator tile held in registers.
+// Fused epilogues of the bf16 GEMM kernel (gemm.cu) and the e4m3 GEMM kernel (fp8.cu). One call handles one thread's wgmma
+// fragment of a 128 x BN accumulator tile held in registers.
 #pragma once
 #include "mmdp_internal.h"
 #include "ptx.cuh"
@@ -101,16 +101,16 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
                 *reinterpret_cast<uint32_t*>(p.C + (size_t)row * p.ldc + col) = o;
             }
         } else if constexpr (EPI == EPI_SWIGLU) {
-            // tile columns [0,128) = gate rows of W1, [128,256) = up rows of W3 (weights packed interleaved)
+            // tile columns [0,BN/2) = gate rows of W1, [BN/2,BN) = up rows of W3 (weights packed interleaved in BN/2-row blocks)
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                const int col = n_blk * 128 + 8 * j + c0;
+            for (int j = 0; j < BN / 16; ++j) {
+                const int col = n_blk * (BN / 2) + 8 * j + c0;
                 if (col >= p.N / 2) continue;
                 float o[2];
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     const float gg = bf16_round(acc[4 * j + 2 * h + e]);
-                    const float uu = bf16_round(acc[4 * (j + 16) + 2 * h + e]);
+                    const float uu = bf16_round(acc[4 * (j + BN / 16) + 2 * h + e]);
                     const float s = bf16_round(__fdiv_rn(gg, __fadd_rn(1.0f, expf(-gg))));  // silu -> bf16
                     o[e] = __fmul_rn(s, uu);
                 }

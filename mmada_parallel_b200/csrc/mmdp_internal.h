@@ -75,7 +75,7 @@ inline cudaError_t launch_ex(void (*kernel)(KArgs...), dim3 grid, dim3 block, si
 // 128-byte swizzle (box_cols must be 64), out-of-bounds elements read as zero.
 int make_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
                       uint32_t box_cols);
-// generic: elem_bytes 2 (bf16, box_cols 64) or 4 (fp32/tf32, box_cols 32)
+// generic: elem_bytes 1 (e4m3, box_cols 128), 2 (bf16, box_cols 64) or 4 (fp32/tf32, box_cols 32)
 int make_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, uint64_t rows, uint64_t cols, uint64_t ld,
                  uint32_t box_rows, uint32_t box_cols);
 
@@ -116,6 +116,17 @@ struct GemmScatter {
 int gemm_bf16(int epi, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int ldw, int M, int N, int K,
               __nv_bfloat16* C, int ldc, const __nv_bfloat16* resid, int ldr, const QkvRopeArgs* qa,
               cudaStream_t stream, const GemmScatter* sc = nullptr);
+
+// tile order of the persistent GEMMs (gemm.cu): the m-tile group size for M rows
+int gemm_group_m(int M);
+
+// FP8 (e4m3) path (fp8.cu). quantize_fp8: x bf16 [rows, K] (row stride ldx) -> q e4m3 [rows, K] (row stride ldq) and fp32
+// scales [K / group][rows]; group divides K and is a multiple of 128. gemm_fp8: A e4m3 [M, K] with scales sa [K/128][M],
+// W e4m3 [N, K] with row scales sw [N]; epilogues PLAIN, RESID, SWIGLU (W13 interleaved in 64-row blocks), QKVROPE.
+int quantize_fp8(const __nv_bfloat16* x, int ldx, int rows, int K, int group, uint8_t* q, int ldq, float* scales,
+                 cudaStream_t stream);
+int gemm_fp8(int epi, const uint8_t* A, int lda, const float* sa, const uint8_t* W, int ldw, const float* sw, int M, int N,
+             int K, __nv_bfloat16* C, int ldc, const __nv_bfloat16* resid, int ldr, const QkvRopeArgs* qa, cudaStream_t stream);
 
 int gemm_pair_mode();
 void set_gemm_pair_mode(int on);

@@ -164,7 +164,7 @@ int make_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, uint64_t ro
                  uint32_t box_rows, uint32_t box_cols) {
     EncodeTiledFn fn = encode_fn();
     if (!fn) return set_error("cuTensorMapEncodeTiled not available (no CUDA driver / no GPU)");
-    if (elem_bytes != 2 && elem_bytes != 4) return set_error("tmap: element size must be 2 (bf16) or 4 (fp32)");
+    if (elem_bytes != 1 && elem_bytes != 2 && elem_bytes != 4) return set_error("tmap: element size must be 1 (e4m3), 2 (bf16) or 4 (fp32)");
     if (box_cols * (uint32_t)elem_bytes != 128) return set_error("tmap: box must be exactly one 128-byte swizzle atom wide");
     if (box_rows == 0 || box_rows > 256) return set_error("tmap: box_rows out of range");
     const TmapKey key{base, rows, cols, ld, box_rows, box_cols, elem_bytes};
@@ -180,7 +180,9 @@ int make_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, uint64_t ro
     cuuint64_t gstride[1] = {ld * (uint64_t)elem_bytes};
     cuuint32_t box[2] = {box_cols, box_rows};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = fn(out, elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), gdim, gstride, box, estr,
+    const CUtensorMapDataType dt = elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                   : (elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32);
+    CUresult r = fn(out, dt, 2, const_cast<void*>(base), gdim, gstride, box, estr,
                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS)

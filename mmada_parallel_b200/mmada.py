@@ -22,8 +22,9 @@ from .schedule import cosine_schedule, get_num_transfer_tokens_m, image_generati
 
 
 class MMadaModelLM(LLaDAForMultiModalGeneration):
-    def __init__(self, config, max_seq_len: Optional[int] = None, max_batch: int = 2, device: str = "cuda:0"):
-        super().__init__(config, max_seq_len=max_seq_len, max_batch=max(2, max_batch), device=device)
+    def __init__(self, config, max_seq_len: Optional[int] = None, max_batch: int = 2, device: str = "cuda:0",
+                 precision: str = "bf16"):
+        super().__init__(config, max_seq_len=max_seq_len, max_batch=max(2, max_batch), device=device, precision=precision)
 
     def forward(self, input_ids=None, **kw):
         """M calls the backbone directly: `self(ids).logits` (modeling_mmada.py:172)."""

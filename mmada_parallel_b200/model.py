@@ -36,6 +36,8 @@ def rope_tables(head_dim: int, theta: float, seq_len: int) -> Tuple[torch.Tensor
     return freqs.cos().contiguous(), freqs.sin().contiguous()
 
 
+_PRECISIONS = {"bf16": _lib.PRECISION_BF16, "fp8": _lib.PRECISION_FP8}
+
 _BLOCK_KEYS = ("q_proj", "k_proj", "v_proj", "attn_out", "ff_proj", "up_proj", "ff_out", "attn_norm", "ff_norm")
 
 
@@ -64,7 +66,12 @@ class LLaDAForMultiModalGeneration:
     """H100-native drop-in for the reference's inference-time model object (variant A wrapper and, through
     `MMadaModelLM` in mmada.py, variant M)."""
 
-    def __init__(self, config, max_seq_len: Optional[int] = None, max_batch: int = 3, device: str = "cuda:0"):
+    def __init__(self, config, max_seq_len: Optional[int] = None, max_batch: int = 3, device: str = "cuda:0",
+                 precision: str = "bf16"):
+        """precision: "bf16" (default) or "fp8" - the four linears of every block in e4m3 with per-row weight scales and 1 x 128
+        activation groups (include/mmdp.h, mmdp_model_create_ex); everything else stays bf16."""
+        if precision not in _PRECISIONS:
+            raise ValueError(f"precision must be one of {sorted(_PRECISIONS)}, got {precision!r}")
         if not torch.cuda.is_available():
             raise _lib.MmdpError("mmada_parallel_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.config = config
@@ -80,11 +87,12 @@ class LLaDAForMultiModalGeneration:
         self.rope_theta = float(g("rope_theta", 10000.0))
         self.max_seq_len = int(max_seq_len or g("max_sequence_length", 4096))
         self.max_batch = int(max_batch)
+        self.precision = precision
         check_supported_config(config, self.n_heads)
         cfg = _lib.ModelConfig(self.d_model, self.n_heads, self.n_layers, self.mlp_hidden, self.vocab_rows,
                                self.max_seq_len, self.max_batch, self.rms_eps)
         handle = C.c_void_p()
-        check(lib.mmdp_model_create(C.byref(cfg), C.byref(handle)))
+        check(lib.mmdp_model_create_ex(C.byref(cfg), _PRECISIONS[precision], C.byref(handle)))
         self._h = handle
         cos, sin = rope_tables(self.d_model // self.n_heads, self.rope_theta, self.max_seq_len)
         check(lib.mmdp_model_set_rope(self._h, cos.data_ptr(), sin.data_ptr(), self.max_seq_len, stream_ptr()))
@@ -150,13 +158,14 @@ class LLaDAForMultiModalGeneration:
 
     @classmethod
     def from_pretrained(cls, path: str, torch_dtype=torch.bfloat16, device_map=None, max_batch: int = 3,
-                        device: str = "cuda:0", **_) -> "LLaDAForMultiModalGeneration":
-        """Loads a HF checkpoint directory (config.json + *.safetensors), mirroring the call at A/inference.py:83-85."""
+                        device: str = "cuda:0", precision: str = "bf16", **_) -> "LLaDAForMultiModalGeneration":
+        """Loads a HF checkpoint directory (config.json + *.safetensors), mirroring the call at A/inference.py:83-85.
+        With precision="fp8" the bf16 linears are quantised on the device as they load."""
         from safetensors import safe_open
 
         with open(os.path.join(path, "config.json")) as f:
             cfg = SimpleNamespace(**json.load(f))
-        m = cls(cfg, max_batch=max_batch, device=device)
+        m = cls(cfg, max_batch=max_batch, device=device, precision=precision)
         files = sorted(f for f in os.listdir(path) if f.endswith(".safetensors"))
         if not files:
             raise FileNotFoundError(f"no *.safetensors under {path}")
