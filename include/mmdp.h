@@ -279,6 +279,47 @@ MMDP_API int mmdp_vqdec_decode(mmdp_vqdec* d, const int64_t* ids, int B, int h, 
 MMDP_API int mmdp_vqenc_create(const mmdp_vqdec_config* cfg, mmdp_vqdec** out);
 MMDP_API int mmdp_vqenc_encode(mmdp_vqdec* enc, const float* pixels_nchw, int B, int H, int W, int64_t* ids_out, void* stream);
 
+/* ---- aMUSEd VQ-VAE context: diffusers.VQModel (variant A's tokenizer; autoencoders/vq_model.py, Encoder / Decoder in
+ * autoencoders/vae.py) -------------------------------------------------------------------------------------------------
+ * Same opaque type and machinery as the MagViT contexts: parameters are loaded with mmdp_vqdec_set_weight under diffusers'
+ * names ("encoder.down_blocks.0.resnets.1.conv1.weight", "decoder.mid_block.attentions.0.to_q.weight", "quant_conv.bias",
+ * "post_quant_conv.weight", "quantize.embedding.weight", ...; Linear weights [C, C], conv OIHW), checked with
+ * mmdp_vqdec_missing and freed with mmdp_vqdec_destroy. Supported: DownEncoderBlock2D / UpDecoderBlock2D, GroupNorm with 32
+ * groups (eps 1e-6), SiLU, optional single-head mid-block attention, vq_embed_dim == latent_channels.
+ * Any latent grid h x w with h * w <= max_latent_cells is accepted (pixels = latent * 2^(n_levels-1)); the activation
+ * buffers are sized for the worst padded area over those grids. */
+typedef struct {
+    int32_t in_channels;              /* 3 */
+    int32_t out_channels;             /* 3 */
+    int32_t n_levels;                 /* len(block_out_channels), <= 8 */
+    int32_t block_out_channels[8];    /* (128, 256, 256, 512, 768), each a multiple of 32 */
+    int32_t layers_per_block;         /* 2: encoder blocks have 2 resnets, decoder blocks 3 */
+    int32_t latent_channels;          /* 64, <= 256 */
+    int32_t num_vq_embeddings;        /* 8192 */
+    int32_t mid_block_add_attention;  /* 0 / 1 */
+    int32_t max_batch;
+    int32_t max_latent_cells;         /* 1024 = 32 x 32, 64 x 16, ... */
+} mmdp_vqmodel_config;
+
+MMDP_API int mmdp_vqmodel_create(const mmdp_vqmodel_config* cfg, mmdp_vqdec** out);
+/* VQModel.decode: exactly one of ids / latents_nchw is given.
+ *   ids int64 [B, h*w] (row-major (y, x)) -> quantize.get_codebook_entry (an id outside [0, num_vq_embeddings) raises bit 0
+ *   of mmdp_vqmodel_error_flags and decodes as a zero vector), or latents fp32 [B, latent_channels, h, w] taken as given;
+ *   then post_quant_conv and the Decoder -> out fp32 [B, out_channels, h * 2^(n_levels-1), w * 2^(n_levels-1)]. */
+MMDP_API int mmdp_vqmodel_decode(mmdp_vqdec* d, const int64_t* ids, const float* latents_nchw, int B, int h, int w, float* out_nchw,
+                                 void* stream);
+/* VQModel.encode: pixels fp32 [B, in_channels, H, W] (H, W multiples of 2^(n_levels-1)) -> Encoder -> quant_conv ->
+ * latents fp32 [B, latent_channels, H / 2^(n_levels-1), W / 2^(n_levels-1)]. */
+MMDP_API int mmdp_vqmodel_encode(mmdp_vqdec* d, const float* pixels_nchw, int B, int H, int W, float* latents_nchw, void* stream);
+/* Sticky device-side error flags of the decodes issued so far, read and cleared (SYNCHRONISES `stream`): bit 0 = an id was
+ * outside the codebook (nn.Embedding raises IndexError). */
+MMDP_API int mmdp_vqmodel_error_flags(mmdp_vqdec* d, int32_t* flags_host, void* stream);
+/* VectorQuantizer's argmin (torch.argmin(torch.cdist(z, codebook))): latents fp32 [B, C, h, w], codebook fp32 [n_codes, C]
+ * (C <= 256) -> ids_out int64 [B*h*w] in (b, y, x) order, the code of least squared fp32 distance sum_c (z_c - e_c)^2 (summed
+ * over c in order), lowest index on ties; zq_nchw (nullable) fp32 [B, C, h, w] = the chosen codebook rows. */
+MMDP_API int mmdp_vq_nearest(const float* latents_nchw, const float* codebook, int B, int C, int h, int w, int n_codes,
+                             int64_t* ids_out, float* zq_nchw, void* stream);
+
 /* ---- whole-model context (LLaDAModel.forward, modeling_llada.py:1201-1415) ----------------------------------- */
 typedef struct mmdp_model mmdp_model;
 

@@ -43,6 +43,13 @@ class VqDecConfig(C.Structure):
                 ("latent_w", C.c_int32)]
 
 
+class VqModelConfig(C.Structure):
+    _fields_ = [("in_channels", C.c_int32), ("out_channels", C.c_int32), ("n_levels", C.c_int32),
+                ("block_out_channels", C.c_int32 * 8), ("layers_per_block", C.c_int32), ("latent_channels", C.c_int32),
+                ("num_vq_embeddings", C.c_int32), ("mid_block_add_attention", C.c_int32), ("max_batch", C.c_int32),
+                ("max_latent_cells", C.c_int32)]
+
+
 class TpLayer(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("wqkv", "wo", "w13", "w2", "attn_norm", "ff_norm")]
 
@@ -116,6 +123,11 @@ SIGNATURES = {
     "mmdp_vqdec_decode": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
     "mmdp_vqenc_create": (_i, [C.POINTER(VqDecConfig), C.POINTER(_vp)]),
     "mmdp_vqenc_encode": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
+    "mmdp_vqmodel_create": (_i, [C.POINTER(VqModelConfig), C.POINTER(_vp)]),
+    "mmdp_vqmodel_decode": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
+    "mmdp_vqmodel_encode": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
+    "mmdp_vqmodel_error_flags": (_i, [_vp, C.POINTER(C.c_int32), _vp]),
+    "mmdp_vq_nearest": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "mmdp_model_create": (_i, [C.POINTER(ModelConfig), C.POINTER(_vp)]),
     "mmdp_model_create_ex": (_i, [C.POINTER(ModelConfig), _i, C.POINTER(_vp)]),
     "mmdp_model_destroy": (None, [_vp]),

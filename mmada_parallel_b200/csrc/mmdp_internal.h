@@ -93,6 +93,12 @@ int nchw_to_padded(const float* x, float* y, int B, int C, int Cpad, int H, int 
 int downsample_pick(const float* src, float* dst, int B, int C, int H, int W, cudaStream_t stream);
 int lfq_indices(const float* z, int64_t* ids, int B, int h, int w, int bits, int ld, cudaStream_t stream);
 int padded_to_nchw(const float* x, float* y, int B, int C, int ld, int H, int W, cudaStream_t stream);
+// learned codebook of the aMUSEd VQ-VAE (vq_codebook.cu). codebook_to_padded: ids outside [0, n_codes) raise bit 0 of *err
+// and give zero vectors. vq_nearest: argmin_k |z - e_k|^2 in exact fp32, lowest index on ties; zq (nullable) NCHW.
+int codebook_to_padded(const int64_t* ids, const float* cb, float* z, int B, int h, int w, int C, int Cpad, int64_t n_codes,
+                       int* err, cudaStream_t stream);
+int vq_nearest(const float* z, const float* cb, int B, int C, int h, int w, int n_codes, int64_t* ids, float* zq,
+               cudaStream_t stream);
 
 struct QkvRopeArgs {
     __nv_bfloat16* q;       // [B*L, d_model]   rotary applied, head h at columns [128h, 128h+128)
