@@ -183,6 +183,11 @@ MMDP_API int mmdp_resid_add_f32(uint16_t* x, int ldx, const float* partial, int 
  * they are multiplied by probabilities that are exactly or nearly (2^-126) zero. */
 MMDP_API int mmdp_attention(const uint16_t* q, const uint16_t* k, const uint16_t* vt, uint16_t* out, int B, int n_heads, int L,
                    int Lpad, float scale, void* stream);
+/* The same over a PACKED variable-length batch: n_seg (1..64) sequences of seg_len[i] (host int32) rows laid end to end.
+ * q,k,out: [sum seg_len, n_heads*128]; vt: [n_seg, n_heads, 128, Lpad] with Lpad >= every seg_len, Lpad % 8 == 0. Sequence i
+ * attends to its own keys only; its pad columns vt[i, ..., seg_len[i]:Lpad] must hold finite values (they meet P == 0). */
+MMDP_API int mmdp_attention_packed(const uint16_t* q, const uint16_t* k, const uint16_t* vt, uint16_t* out, int n_seg, const int32_t* seg_len,
+                                   int n_heads, int Lpad, float scale, void* stream);
 
 /* RMSLayerNorm.forward (modeling_llada.py:315-329). rows (nullable int32[M]) gathers input rows. */
 MMDP_API int mmdp_rmsnorm(const uint16_t* x, int ldx, const int32_t* rows, const uint16_t* weight, uint16_t* y, int ldy, int M,
@@ -371,6 +376,15 @@ MMDP_API int mmdp_model_forward(mmdp_model* m, const int64_t* ids, int B, int L,
 MMDP_API int mmdp_model_forward_window(mmdp_model* m, const int64_t* ids, int B, int L, const int32_t* rows_a, int n_a, uint16_t* out_a,
                               const int32_t* rows_b, int n_b, int col0_b, int ncols_b, uint16_t* out_b, int row_lo, int row_hi,
                               void* stream);
+/* One forward over a PACKED variable-length batch: n_seg sequences (1 <= n_seg <= max_batch, and at most 64) of seg_len[i]
+ * tokens (host int32, each in [1, max_seq_len]) laid end to end in ids [sum seg_len] (int64). Every sequence is computed as if
+ * it were alone: attention never crosses into another sequence and rotary positions restart at 0 in each. rows_a / rows_b are
+ * packed row indices (sequence i's token p is row sum_{j<i} seg_len[j] + p); the head outputs are those of mmdp_model_forward.
+ * The last block runs on all rows (no row window). Bad sizes return an error before anything is launched; token ids outside
+ * the vocabulary raise bit 0 of the error flags. Works on bf16 and FP8 contexts. */
+MMDP_API int mmdp_model_forward_packed(mmdp_model* m, const int64_t* ids, int n_seg, const int32_t* seg_len, const int32_t* rows_a,
+                                       int n_a, uint16_t* out_a, const int32_t* rows_b, int n_b, int col0_b, int ncols_b, uint16_t* out_b,
+                                       void* stream);
 
 /* Debug/testing: copy of the residual stream after `layer` layers is kept when enabled (device pointer returned). */
 MMDP_API const uint16_t* mmdp_model_hidden(mmdp_model* m);

@@ -105,6 +105,7 @@ SIGNATURES = {
     "mmdp_qkv_rope_tp": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mmdp_resid_add_f32": (_i, [_vp, _i, _vp, _i, _i, _i, _vp]),
     "mmdp_attention": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp]),
+    "mmdp_attention_packed": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _f, _vp]),
     "mmdp_rmsnorm": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _f, _vp]),
     "mmdp_embed": (_i, [_vp, _vp, _vp, _i, _i, _i64, _vp]),
     "mmdp_text_step": (_i, [_vp, _vp, _i64, _i, _i, _f, _vp, _i64, _f, _vp, _i64, _i, _vp, _vp, _vp]),
@@ -135,6 +136,7 @@ SIGNATURES = {
     "mmdp_model_set_rope": (_i, [_vp, _vp, _vp, _i, _vp]),
     "mmdp_model_forward": (_i, [_vp, _vp, _i, _i, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp, _vp]),
     "mmdp_model_forward_window": (_i, [_vp, _vp, _i, _i, _vp, _i, _vp, _vp, _i, _i, _i, _vp, _i, _i, _vp]),
+    "mmdp_model_forward_packed": (_i, [_vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp, _vp]),
     "mmdp_model_forward_cached": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "mmdp_model_hidden": (_vp, [_vp]),
     "mmdp_model_error_flags": (_i, [_vp, C.POINTER(C.c_int32), _vp]),
@@ -243,6 +245,17 @@ def attention(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, B: int, n_head
     require_cuda(q, k, vt)
     out = torch.empty_like(q)
     check(lib.mmdp_attention(ptr(q), ptr(k), ptr(vt), ptr(out), B, n_heads, L, vt.shape[-1], scale, stream_ptr()))
+    return out
+
+
+def attention_packed(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, seq_lens, n_heads: int, scale: float) -> torch.Tensor:
+    """Attention over a packed batch: q, k [sum(seq_lens), n_heads * 128]; vt [len(seq_lens), n_heads, 128, Lpad] with zero
+    (or finite) pad columns. Each sequence attends to its own keys only."""
+    require_cuda(q, k, vt)
+    lens = (C.c_int32 * len(seq_lens))(*[int(x) for x in seq_lens])
+    out = torch.empty_like(q)
+    check(lib.mmdp_attention_packed(ptr(q), ptr(k), ptr(vt), ptr(out), len(seq_lens), lens, n_heads, vt.shape[-1], scale,
+                                    stream_ptr()))
     return out
 
 

@@ -24,6 +24,23 @@ __global__ void lfq_kernel(const int64_t* __restrict__ ids, float* __restrict__ 
     for (int c = 0; c < bits; ++c) zq[((size_t)b * bits + c) * N + n] = ((id >> (bits - 1 - c)) & 1) ? 1.0f : -1.0f;
 }
 
+__global__ void packed_row_map_kernel(const __grid_constant__ SegTable segs, int2* __restrict__ seg_pos) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= segs.start[segs.n]) return;
+    int s = 0;
+    for (int i = 1; i < segs.n; ++i)
+        if (r >= segs.start[i]) s = i;
+    seg_pos[r] = make_int2(s, r - segs.start[s]);
+}
+
+int packed_row_map(const SegTable& segs, int2* seg_pos, cudaStream_t stream) {
+    const int M = segs.start[segs.n];
+    LaunchScope ls(LK_ROW, 8.0 * M, stream);
+    packed_row_map_kernel<<<(M + 255) / 256, 256, 0, stream>>>(segs, seg_pos);
+    MMDP_CUDA(cudaGetLastError());
+    return 0;
+}
+
 int lfq_decode(const int64_t* ids, float* zq, int B, int N, int bits, cudaStream_t stream) {
     if (B <= 0 || N <= 0) return 0;
     if (bits <= 0 || bits > 62) return set_error("lfq_decode: bits out of range");
@@ -62,7 +79,11 @@ struct mmdp_model {
     int Mmax = 0, Lpad_max = 0;
     bf16 *x = nullptr, *xn = nullptr, *q = nullptr, *k = nullptr, *vt = nullptr, *att = nullptr, *h = nullptr, *xr = nullptr;
     int* err_flag = nullptr;  // device: bit 0 = token id out of range, bit 1 = logits row index out of range
-    int vt_B = 0, vt_Lpad = 0, vt_L = 0;  // layout / length the vt buffer was last zeroed for
+    // V^T pad rule (vt_prepare): vt_Lpad = column stride of the layout the buffer was last zeroed for, vt_len[s] = columns
+    // of block s written since then
+    int vt_Lpad = 0;
+    std::vector<int> vt_len;
+    int2* seg_pos = nullptr;  // packed forward: (sequence, position) of every packed row
     int precision = MMDP_PRECISION_BF16;
     uint8_t* a8 = nullptr;  // FP8: the quantised input of the current linear, [M, K] e4m3
     float* as = nullptr;    // FP8: its scales, [K / 128][M]
@@ -123,6 +144,15 @@ MMDP_API int mmdp_attention(const uint16_t* q, const uint16_t* k, const uint16_t
                    int Lpad, float scale, void* stream) {
     return attention_fwd((const bf16*)q, (const bf16*)k, (const bf16*)vt, (bf16*)out, B, n_heads, L, Lpad, scale,
                          (cudaStream_t)stream);
+}
+
+MMDP_API int mmdp_attention_packed(const uint16_t* q, const uint16_t* k, const uint16_t* vt, uint16_t* out, int n_seg, const int32_t* seg_len,
+                                   int n_heads, int Lpad, float scale, void* stream) {
+    if (!seg_len || n_seg <= 0 || n_seg > kMaxSegs) return set_error("mmdp_attention_packed: %d sequences (1 to %d)", n_seg, kMaxSegs);
+    SegTable segs{};
+    segs.n = n_seg;
+    for (int i = 0; i < n_seg; ++i) segs.start[i + 1] = segs.start[i] + seg_len[i];
+    return attention_packed_fwd((const bf16*)q, (const bf16*)k, (const bf16*)vt, (bf16*)out, segs, n_heads, Lpad, scale, (cudaStream_t)stream);
 }
 
 MMDP_API int mmdp_rmsnorm(const uint16_t* x, int ldx, const int32_t* rows, const uint16_t* weight, uint16_t* y, int ldy, int M,
@@ -407,6 +437,8 @@ MMDP_API int mmdp_model_create_ex(const mmdp_model_config* c, int precision, mmd
     rc |= dev_alloc(m, (void**)&m->cos_tab, (size_t)c->max_seq_len * 64 * 4);
     rc |= dev_alloc(m, (void**)&m->sin_tab, (size_t)c->max_seq_len * 64 * 4);
     rc |= dev_alloc(m, (void**)&m->err_flag, sizeof(int));
+    rc |= dev_alloc(m, (void**)&m->seg_pos, Mm * sizeof(int2));
+    m->vt_len.assign(c->max_batch, 0);
     if (!rc && cudaMemset(m->err_flag, 0, sizeof(int)) != cudaSuccess) rc = set_error("mmdp_model_create: cudaMemset failed");
     if (rc) {
         mmdp_model_destroy(m);
@@ -550,6 +582,44 @@ static int block_linear(mmdp_model* m, const LayerWeights& l, int which, int epi
     return gemm_fp8(epi, m->a8, K, m->as, W, K, sw, M, N, K, C, ldc, R, ldr, qa, s);
 }
 
+// V^T pad rule. Block s of m->vt ([max_batch][H][128][Lpad], the batch row or the packed sequence s) is read by the P·V MMA
+// up to its padded length, and its columns [L_s, Lpad) meet P == 0 there: they must be finite zeros. A forward over blocks
+// [0, n) with lengths lens[] at column stride Lpad zeroes the whole buffer when the stride changes or when one of its blocks
+// holds columns beyond its new length (a longer forward wrote them); otherwise every column it reads past L_s is still zero.
+static int vt_prepare(mmdp_model* m, int n, const int* lens, int Lpad, cudaStream_t s) {
+    bool zero = m->vt_Lpad != Lpad;
+    for (int i = 0; i < n && !zero; ++i) zero = m->vt_len[i] > lens[i];
+    if (zero) {
+        MMDP_CUDA(cudaMemsetAsync(m->vt, 0, (size_t)m->cfg.max_batch * m->cfg.d_model * m->Lpad_max * 2, s));
+        m->vt_len.assign(m->cfg.max_batch, 0);
+        m->vt_Lpad = Lpad;
+    }
+    for (int i = 0; i < n; ++i) m->vt_len[i] = lens[i];
+    return 0;
+}
+
+// ln_f + LM head on the gathered rows (rows_a: all V columns; rows_b: columns [col0_b, col0_b + ncols_b)) of the M rows in
+// m->x. row_lo / row_hi / L: the last block's row window (0: none); a row outside it raises bit 2 of the error flag.
+static int head_rows(mmdp_model* m, int M, const int32_t* rows_a, int n_a, uint16_t* out_a, const int32_t* rows_b, int n_b,
+                     int col0_b, int ncols_b, uint16_t* out_b, int row_lo, int row_hi, int L, cudaStream_t s) {
+    const mmdp_model_config& c = m->cfg;
+    const int d = c.d_model, V = c.vocab_size;
+    if (n_a > 0) {
+        if (!rows_a || !out_a) return set_error("mmdp_model_forward: rows_a/out_a null");
+        if (n_a > m->Mmax) return set_error("mmdp_model_forward: too many rows_a");
+        if (rmsnorm_rows(m->x, d, rows_a, m->ln_f, m->xr, d, n_a, d, c.rms_eps, s, M, m->err_flag, row_lo, row_hi, L)) return -1;
+        if (gemm_bf16(EPI_PLAIN, m->xr, d, m->head, d, n_a, V, d, (bf16*)out_a, V, nullptr, 0, nullptr, s)) return -1;
+    }
+    if (n_b > 0) {
+        if (!rows_b || !out_b) return set_error("mmdp_model_forward: rows_b/out_b null");
+        if (n_a + n_b > m->Mmax) return set_error("mmdp_model_forward: too many rows_a + rows_b");
+        bf16* xr_b = m->xr + (size_t)n_a * d;
+        if (rmsnorm_rows(m->x, d, rows_b, m->ln_f, xr_b, d, n_b, d, c.rms_eps, s, M, m->err_flag, row_lo, row_hi, L)) return -1;
+        if (gemm_bf16(EPI_PLAIN, xr_b, d, m->head + (size_t)col0_b * d, d, n_b, ncols_b, d, (bf16*)out_b, ncols_b, nullptr, 0, nullptr, s)) return -1;
+    }
+    return 0;
+}
+
 static int model_forward(mmdp_model* m, const int64_t* ids, int B, int L, uint16_t* full_logits, const int32_t* rows_a,
                          int n_a, uint16_t* out_a, const int32_t* rows_b, int n_b, int col0_b, int ncols_b,
                          uint16_t* out_b, int row_lo, int row_hi, void* stream) {
@@ -564,14 +634,8 @@ static int model_forward(mmdp_model* m, const int64_t* ids, int B, int L, uint16
     const int d = c.d_model, ff = c.mlp_hidden, V = c.vocab_size, H = c.n_heads;
     const int M = B * L;
     const int Lpad = ((L + 7) / 8) * 8;
-    if (m->vt_Lpad != Lpad || L < m->vt_L) {  // (indexing depends on Lpad only; batch rows are disjoint)
-        // pad columns [L, Lpad) of V^T must be zero (they meet P == 0 in the P·V MMA): re-zero when the layout changes or
-        // when L shrinks inside the same Lpad (columns a longer forward wrote would otherwise stay behind)
-        MMDP_CUDA(cudaMemsetAsync(m->vt, 0, (size_t)c.max_batch * d * m->Lpad_max * 2, s));
-        m->vt_B = B;
-        m->vt_Lpad = Lpad;
-    }
-    m->vt_L = L;
+    const std::vector<int> lens(B, L);
+    if (vt_prepare(m, B, lens.data(), Lpad, s)) return -1;
     const float scale = 1.0f / sqrtf(128.0f);
     if (embed_rows(ids, m->wte, m->x, M, d, V, s, m->err_flag)) return -1;
     QkvRopeArgs qa{m->q, m->k, m->vt, m->cos_tab, m->sin_tab, L, Lpad, d, H};
@@ -607,20 +671,8 @@ static int model_forward(mmdp_model* m, const int64_t* ids, int B, int L, uint16
         if (rmsnorm(m->x, d, m->ln_f, m->xn, d, M, d, c.rms_eps, s)) return -1;
         if (gemm_bf16(EPI_PLAIN, m->xn, d, m->head, d, M, V, d, (bf16*)full_logits, V, nullptr, 0, nullptr, s)) return -1;
     }
-    if (n_a > 0) {
-        if (!rows_a || !out_a) return set_error("mmdp_model_forward: rows_a/out_a null");
-        if (n_a > m->Mmax) return set_error("mmdp_model_forward: too many rows_a");
-        if (rmsnorm_rows(m->x, d, rows_a, m->ln_f, m->xr, d, n_a, d, c.rms_eps, s, M, m->err_flag, window ? row_lo : 0, window ? row_hi : 0, window ? L : 0)) return -1;
-        if (gemm_bf16(EPI_PLAIN, m->xr, d, m->head, d, n_a, V, d, (bf16*)out_a, V, nullptr, 0, nullptr, s)) return -1;
-    }
-    if (n_b > 0) {
-        if (!rows_b || !out_b) return set_error("mmdp_model_forward: rows_b/out_b null");
-        if (n_a + n_b > m->Mmax) return set_error("mmdp_model_forward: too many rows_a + rows_b");
-        bf16* xr_b = m->xr + (size_t)n_a * d;
-        if (rmsnorm_rows(m->x, d, rows_b, m->ln_f, xr_b, d, n_b, d, c.rms_eps, s, M, m->err_flag, window ? row_lo : 0, window ? row_hi : 0, window ? L : 0)) return -1;
-        if (gemm_bf16(EPI_PLAIN, xr_b, d, m->head + (size_t)col0_b * d, d, n_b, ncols_b, d, (bf16*)out_b, ncols_b, nullptr, 0, nullptr, s)) return -1;
-    }
-    return 0;
+    return head_rows(m, M, rows_a, n_a, out_a, rows_b, n_b, col0_b, ncols_b, out_b, window ? row_lo : 0, window ? row_hi : 0,
+                     window ? L : 0, s);
 }
 
 // Token-cache forward (reference: LLaDAModelLM.forward(input_ids, use_cache=True, to_compute_mask=mask, cat=key),
@@ -644,6 +696,48 @@ MMDP_API int mmdp_model_forward_window(mmdp_model* m, const int64_t* ids, int B,
                               const int32_t* rows_b, int n_b, int col0_b, int ncols_b, uint16_t* out_b, int row_lo, int row_hi,
                               void* stream) {
     return model_forward(m, ids, B, L, nullptr, rows_a, n_a, out_a, rows_b, n_b, col0_b, ncols_b, out_b, row_lo, row_hi, stream);
+}
+
+MMDP_API int mmdp_model_forward_packed(mmdp_model* m, const int64_t* ids, int n_seg, const int32_t* seg_len, const int32_t* rows_a,
+                                       int n_a, uint16_t* out_a, const int32_t* rows_b, int n_b, int col0_b, int ncols_b, uint16_t* out_b,
+                                       void* stream) {
+    if (!m || !ids || !seg_len) return set_error("mmdp_model_forward_packed: null argument");
+    const mmdp_model_config& c = m->cfg;
+    if (n_seg <= 0 || n_seg > c.max_batch || n_seg > kMaxSegs)
+        return set_error("mmdp_model_forward_packed: %d sequences outside [1, %d] (max_batch, at most %d)", n_seg, c.max_batch, kMaxSegs);
+    SegTable segs{};
+    segs.n = n_seg;
+    int Lmax = 0;
+    for (int i = 0; i < n_seg; ++i) {
+        if (seg_len[i] <= 0 || seg_len[i] > c.max_seq_len)
+            return set_error("mmdp_model_forward_packed: sequence %d has length %d (max_seq_len=%d)", i, seg_len[i], c.max_seq_len);
+        segs.start[i + 1] = segs.start[i] + seg_len[i];
+        Lmax = seg_len[i] > Lmax ? seg_len[i] : Lmax;
+    }
+    if (Lmax > m->rope_len) return set_error("mmdp_model_forward_packed: rotary table covers %d positions, need %d", m->rope_len, Lmax);
+    if (n_b > 0 && (col0_b < 0 || ncols_b <= 0 || col0_b + ncols_b > c.vocab_size || (ncols_b % 8)))
+        return set_error("mmdp_model_forward_packed: bad column window [%d,+%d)", col0_b, ncols_b);
+    cudaStream_t s = (cudaStream_t)stream;
+    const int d = c.d_model, ff = c.mlp_hidden, V = c.vocab_size, H = c.n_heads;
+    const int M = segs.start[n_seg];
+    const int Lpad = ((Lmax + 7) / 8) * 8;
+    if (vt_prepare(m, n_seg, seg_len, Lpad, s)) return -1;
+    if (packed_row_map(segs, m->seg_pos, s)) return -1;
+    const float scale = 1.0f / sqrtf(128.0f);
+    if (embed_rows(ids, m->wte, m->x, M, d, V, s, m->err_flag)) return -1;
+    QkvRopeArgs qa{m->q, m->k, m->vt, m->cos_tab, m->sin_tab, Lmax, Lpad, d, H};
+    qa.seg_pos = m->seg_pos;
+    for (int li = 0; li < c.n_layers; ++li) {
+        const LayerWeights& l = m->layers[li];
+        if (rmsnorm(m->x, d, l.attn_norm, m->xn, d, M, d, c.rms_eps, s)) return -1;
+        if (block_linear(m, l, LIN_QKV, EPI_QKVROPE_PACKED, m->xn, d, M, nullptr, 0, nullptr, 0, &qa, s)) return -1;
+        if (attention_packed_fwd(m->q, m->k, m->vt, m->att, segs, H, Lpad, scale, s)) return -1;
+        if (block_linear(m, l, LIN_O, EPI_RESID, m->att, d, M, m->x, d, m->x, d, nullptr, s)) return -1;
+        if (rmsnorm(m->x, d, l.ff_norm, m->xn, d, M, d, c.rms_eps, s)) return -1;
+        if (block_linear(m, l, LIN_13, EPI_SWIGLU, m->xn, d, M, m->h, ff, nullptr, 0, nullptr, s)) return -1;
+        if (block_linear(m, l, LIN_2, EPI_RESID, m->h, ff, M, m->x, d, m->x, d, nullptr, s)) return -1;
+    }
+    return head_rows(m, M, rows_a, n_a, out_a, rows_b, n_b, col0_b, ncols_b, out_b, 0, 0, 0, s);
 }
 
 MMDP_API int mmdp_model_forward_cached(mmdp_model* m, const int64_t* ids, int B, int L, int Tq, const int32_t* pos_map, uint16_t* kcache,

@@ -5,7 +5,9 @@
 //   * S = Q K^T with wgmma m64n128k16 (both operands from shared memory), the online softmax on the register fragment
 //     (a query row is spread over the four lanes of a quad), P rounded to bf16 in registers and fed straight back as the A
 //     operand of O += P V (wgmma with A from registers, B = V^T from shared memory); O stays in registers for the whole loop;
-//   * the tiles of a partial last wave are cut along the keys and merged by attention_combine_kernel (see attention_fwd).
+//   * the tiles of a partial last wave are cut along the keys and merged by attention_combine_kernel (see attention_fwd);
+//   * attention_packed_kernel runs the same body over a packed variable-length batch: work items enumerate
+//     (sequence, head, query tile), each sequence attends to its own keys only (attention_packed_fwd).
 #include "mmdp_internal.h"
 #include "ptx.cuh"
 
@@ -33,11 +35,20 @@ __device__ __forceinline__ float ex2_approx(float x) {
     return y;
 }
 
-template <int kBKV>
-__global__ void __launch_bounds__(kAttnThreads, 1)
-attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                 const __grid_constant__ CUtensorMap tmVt, __nv_bfloat16* __restrict__ out, int H, int L, int d_model,
-                 float scale_log2, int n_full, int splits, float* __restrict__ part_ws, int Lq) {
+// Sequence table of a packed launch: sequence s has rows [start[s], start[s + 1]) of q / k / out and the V^T block s; its
+// query tiles are work items [tile0[s], tile0[s + 1]) (before the split of the tail), ordered (head, query tile).
+struct AttnSegs {
+    int n;
+    int start[kMaxSegs + 1];
+    int tile0[kMaxSegs + 1];
+};
+
+// One CTA's work item. kPacked = false: B sequences of L keys / Lq queries each, laid out batch row after batch row (the
+// kernel parameters). kPacked = true: the sequences of `segs`, each with its own length (L = Lq = its length).
+template <int kBKV, bool kPacked>
+__device__ __forceinline__ void attention_body(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmVt,
+                                               __nv_bfloat16* __restrict__ out, int H, int L, int d_model, float scale_log2,
+                                               int n_full, int splits, float* __restrict__ part_ws, int Lq, const AttnSegs* segs) {
     constexpr int kKBytes = AttnCfg<kBKV>::kKBytes, kVBytes = AttnCfg<kBKV>::kVBytes;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -56,22 +67,34 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     // `splits` pieces that each cover a slice of the KV blocks and leave an un-normalised partial (O, m, l) in part_ws for
     // attention_combine_kernel. tile index = (b * H + h) * n_qt + qt.
     // L = number of keys per batch row; Lq = number of query rows per batch row (== L except in the token-cache forward)
-    const int n_qt = (Lq + 127) / 128;
-    const int n_kv_all = (L + kBKV - 1) / kBKV;
+    int n_qt = (Lq + 127) / 128;
+    int n_kv_all = (L + kBKV - 1) / kBKV;
     int tile = blockIdx.x, piece = -1;
     if ((int)blockIdx.x >= n_full) {
         const int t = (int)blockIdx.x - n_full;
         tile = n_full + t / splits;
         piece = t - (t / splits) * splits;
     }
-    const int qt = tile % n_qt, h = (tile / n_qt) % H, b = tile / (n_qt * H);
+    // packed: the tile's sequence (a uniform scan of the small table), its first row and length; keys past its end are masked
+    // through nvalid, query rows past it are not stored
+    int seg = 0, seg0 = 0, tl = tile;
+    if constexpr (kPacked) {
+        for (int i = 1; i < segs->n; ++i)
+            if (tile >= segs->tile0[i]) seg = i;
+        seg0 = segs->start[seg];
+        L = Lq = segs->start[seg + 1] - seg0;
+        n_qt = (Lq + 127) / 128;
+        n_kv_all = (L + kBKV - 1) / kBKV;
+        tl = tile - segs->tile0[seg];
+    }
+    const int qt = tl % n_qt, h = (tl / n_qt) % H, b = kPacked ? seg : tile / (n_qt * H);
     int jb = 0, je = n_kv_all;
     if (piece >= 0) {
         const int per = (n_kv_all + splits - 1) / splits;
         jb = piece * per;
         je = (jb + per < n_kv_all) ? jb + per : n_kv_all;
     }
-    const int n_kv = je - jb;  // >= 1: the host keeps every piece non-empty
+    const int n_kv = je - jb;  // >= 1: the host keeps every piece of every split tile non-empty
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmQ);
@@ -94,7 +117,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
         // ===================== TMA producer: Q, then K(j) and V^T(j) =====================
         setmaxnreg_dec<40>();
         if (warp == 0 && elect_one_sync()) {
-            const int qrow0 = b * Lq + qt * 128;
+            const int qrow0 = (kPacked ? seg0 : b * Lq) + qt * 128;
             mbar_expect_tx(q_full, kQBytes);
             tma_load_2d(sQ, &tmQ, q_full, h * 128, qrow0);
             tma_load_2d(sQ + kQBytes / 2, &tmQ, q_full, h * 128 + 64, qrow0);
@@ -104,8 +127,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
                 const int kv0 = (jb + j) * kBKV;
                 mbar_wait(&k_empty[st], ph ^ 1);
                 mbar_expect_tx(&k_full[st], kKBytes);
-                tma_load_2d(sK + st * kKBytes, &tmK, &k_full[st], h * 128, b * L + kv0);
-                tma_load_2d(sK + st * kKBytes + kKBytes / 2, &tmK, &k_full[st], h * 128 + 64, b * L + kv0);
+                tma_load_2d(sK + st * kKBytes, &tmK, &k_full[st], h * 128, (kPacked ? seg0 : b * L) + kv0);
+                tma_load_2d(sK + st * kKBytes + kKBytes / 2, &tmK, &k_full[st], h * 128 + 64, (kPacked ? seg0 : b * L) + kv0);
                 mbar_wait(&v_empty[st], ph ^ 1);
                 mbar_expect_tx(&v_full[st], kVBytes);
                 tma_load_2d(sV + st * kVBytes, &tmVt, &v_full[st], kv0, (b * H + h) * 128);
@@ -225,7 +248,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
                 *reinterpret_cast<float2*>(slot + (size_t)r * 128 + 8 * jj + c0) = make_float2(o[4 * jj + 2 * hh], o[4 * jj + 2 * hh + 1]);
         } else {
             const float inv_l = 1.0f / l_run[hh];
-            __nv_bfloat16* orow = out + (size_t)(b * Lq + qrow) * d_model + h * 128;
+            __nv_bfloat16* orow = out + (size_t)((kPacked ? seg0 : b * Lq) + qrow) * d_model + h * 128;
 #pragma unroll
             for (int jj = 0; jj < 16; ++jj)
                 *reinterpret_cast<uint32_t*>(orow + 8 * jj + c0) = pack_bf16x2(o[4 * jj + 2 * hh] * inv_l, o[4 * jj + 2 * hh + 1] * inv_l);
@@ -233,17 +256,43 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     }
 }
 
+template <int kBKV>
+__global__ void __launch_bounds__(kAttnThreads, 1)
+attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                 const __grid_constant__ CUtensorMap tmVt, __nv_bfloat16* __restrict__ out, int H, int L, int d_model,
+                 float scale_log2, int n_full, int splits, float* __restrict__ part_ws, int Lq) {
+    attention_body<kBKV, false>(tmQ, tmK, tmVt, out, H, L, d_model, scale_log2, n_full, splits, part_ws, Lq, nullptr);
+}
+
+template <int kBKV>
+__global__ void __launch_bounds__(kAttnThreads, 1)
+attention_packed_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                        const __grid_constant__ CUtensorMap tmVt, __nv_bfloat16* __restrict__ out, int H, int d_model,
+                        float scale_log2, int n_full, int splits, float* __restrict__ part_ws, const __grid_constant__ AttnSegs segs) {
+    attention_body<kBKV, true>(tmQ, tmK, tmVt, out, H, 0, d_model, scale_log2, n_full, splits, part_ws, 0, &segs);
+}
+
 // Merges the `splits` KV-slice partials of one split tile: out = (sum_i w_i O_i) / (sum_i w_i l_i), w_i = 2^((m_i - m) c).
 // One CTA per (split tile, query row), thread = output column.
-__global__ void __launch_bounds__(128)
-attention_combine_kernel(const float* __restrict__ part_ws, __nv_bfloat16* __restrict__ out, int H, int Lq, int d_model,
-                         float scale_log2, int n_full, int splits) {
-    const int n_qt = (Lq + 127) / 128;
+template <bool kPacked>
+__device__ __forceinline__ void attention_combine_body(const float* __restrict__ part_ws, __nv_bfloat16* __restrict__ out, int H,
+                                                       int Lq, int d_model, float scale_log2, int n_full, int splits,
+                                                       const AttnSegs* segs) {
+    int n_qt = (Lq + 127) / 128;
     const int st = blockIdx.x, r = blockIdx.y, c = threadIdx.x;
     pdl_launch_dependents();
     pdl_wait();
     const int tile = n_full + st;
-    const int qt = tile % n_qt, h = (tile / n_qt) % H, b = tile / (n_qt * H);
+    int seg = 0, seg0 = 0, tl = tile;
+    if constexpr (kPacked) {
+        for (int i = 1; i < segs->n; ++i)
+            if (tile >= segs->tile0[i]) seg = i;
+        seg0 = segs->start[seg];
+        Lq = segs->start[seg + 1] - seg0;
+        n_qt = (Lq + 127) / 128;
+        tl = tile - segs->tile0[seg];
+    }
+    const int qt = tl % n_qt, h = (tl / n_qt) % H, b = kPacked ? seg : tile / (n_qt * H);
     const int qrow = qt * 128 + r;
     if (qrow >= Lq) return;
     const float* base = part_ws + (size_t)st * splits * (128 * 128 + 256);
@@ -256,7 +305,19 @@ attention_combine_kernel(const float* __restrict__ part_ws, __nv_bfloat16* __res
         o = fmaf(w, slot[(size_t)r * 128 + c], o);
         l = fmaf(w, slot[128 * 128 + 128 + r], l);
     }
-    out[(size_t)(b * Lq + qrow) * d_model + h * 128 + c] = __float2bfloat16_rn(o / l);
+    out[(size_t)((kPacked ? seg0 : b * Lq) + qrow) * d_model + h * 128 + c] = __float2bfloat16_rn(o / l);
+}
+
+__global__ void __launch_bounds__(128)
+attention_combine_kernel(const float* __restrict__ part_ws, __nv_bfloat16* __restrict__ out, int H, int Lq, int d_model,
+                         float scale_log2, int n_full, int splits) {
+    attention_combine_body<false>(part_ws, out, H, Lq, d_model, scale_log2, n_full, splits, nullptr);
+}
+
+__global__ void __launch_bounds__(128)
+attention_packed_combine_kernel(const float* __restrict__ part_ws, __nv_bfloat16* __restrict__ out, int H, int d_model,
+                                float scale_log2, int n_full, int splits, const __grid_constant__ AttnSegs segs) {
+    attention_combine_body<true>(part_ws, out, H, 0, d_model, scale_log2, n_full, splits, &segs);
 }
 
 // KV-slice partials of the split tail: one buffer per (device, stream), grown on demand
@@ -277,6 +338,51 @@ static int attn_part_workspace(cudaStream_t stream, size_t need, float** out) {
     return 0;
 }
 
+// Partial last wave: tiles % SMs leftover tiles would run alone at the end. Split their KV range over the idle SMs and merge
+// the partials (attention_combine_kernel). kvb_of(t) = number of KV blocks of work item t; every piece of every split tile
+// must be non-empty for its own KV length.
+template <class KvbOf>
+static void plan_split_tail(int tiles, KvbOf kvb_of, int& n_full, int& n_split, int& splits) {
+    const int split_tail = opt(OPT_ATTN_SPLIT_TAIL), slots = num_sms();
+    n_full = tiles; n_split = 0; splits = 1;
+    auto fit_splits = [&](int want, int first) {
+        int sp = want > 8 ? 8 : want;
+        for (int t = first; t < tiles; ++t)
+            if (sp > kvb_of(t) / 2) sp = kvb_of(t) / 2;
+        // no empty piece: piece i covers KV blocks [i * per, (i + 1) * per) with per = ceil(n_kvb / splits)
+        auto empty_piece = [&](int s) {
+            for (int t = first; t < tiles; ++t) {
+                const int n_kvb = kvb_of(t);
+                if ((s - 1) * ((n_kvb + s - 1) / s) >= n_kvb) return true;
+            }
+            return false;
+        };
+        while (sp >= 2 && empty_piece(sp)) --sp;
+        return sp;
+    };
+    if (split_tail && tiles > slots && (tiles % slots) > 0 && (tiles % slots) * 4 <= slots) {
+        n_split = tiles % slots;
+        splits = fit_splits(slots / n_split, tiles - n_split);
+        if (splits >= 2) n_full = tiles - n_split; else { n_split = 0; splits = 1; }
+    } else if (split_tail && tiles * 2 <= slots) {
+        // fewer tiles than half the SMs (a tensor-parallel rank with 4 of the 32 heads): split EVERY tile's KV range so
+        // that the whole machine works on the launch
+        splits = fit_splits(slots / tiles, 0);
+        if (splits >= 2) { n_split = tiles; n_full = 0; } else splits = 1;
+    }
+}
+
+template <class Kernel>
+static int attn_smem_attr(Kernel kernel, int smem, unsigned long long& attr_set) {  // attr_set: bit per device
+    int dev = 0;
+    MMDP_CUDA(cudaGetDevice(&dev));
+    if (!(attr_set >> (dev & 63) & 1ull)) {
+        MMDP_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        attr_set |= 1ull << (dev & 63);
+    }
+    return 0;
+}
+
 template <int kBKV>
 static int attention_launch(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* vt, __nv_bfloat16* out, int B, int H,
                             int L, int Lpad, float scale, cudaStream_t stream, int Lq) {
@@ -289,47 +395,68 @@ static int attention_launch(const __nv_bfloat16* q, const __nv_bfloat16* k, cons
     if (make_tmap_2d_bf16(&tmQ, q, (uint64_t)B * Lq, (uint64_t)d_model, (uint64_t)d_model, 128, 64)) return -1;
     if (make_tmap_2d_bf16(&tmK, k, (uint64_t)B * L, (uint64_t)d_model, (uint64_t)d_model, kBKV, 64)) return -1;
     if (make_tmap_2d_bf16(&tmVt, vt, (uint64_t)B * H * 128, (uint64_t)Lpad, (uint64_t)Lpad, 128, 64)) return -1;
-    const int split_tail = opt(OPT_ATTN_SPLIT_TAIL);
-    // Partial last wave: tiles % SMs leftover tiles would run alone at the end. Split their KV range over the idle SMs and
-    // merge the partials (attention_combine_kernel).
     const int n_qt = (Lq + 127) / 128, n_kvb = (L + kBKV - 1) / kBKV;
-    const int tiles = n_qt * H * B, slots = num_sms();
-    int n_full = tiles, n_split = 0, splits = 1;
-    auto fit_splits = [&](int want) {
-        int sp = want > 8 ? 8 : want;
-        if (sp > n_kvb / 2) sp = n_kvb / 2;
-        // no empty piece: piece i covers KV blocks [i * per, (i + 1) * per) with per = ceil(n_kvb / splits)
-        while (sp >= 2 && (sp - 1) * ((n_kvb + sp - 1) / sp) >= n_kvb) --sp;
-        return sp;
-    };
-    if (split_tail && tiles > slots && (tiles % slots) > 0 && (tiles % slots) * 4 <= slots) {
-        n_split = tiles % slots;
-        splits = fit_splits(slots / n_split);
-        if (splits >= 2) n_full = tiles - n_split; else { n_split = 0; splits = 1; }
-    } else if (split_tail && tiles * 2 <= slots) {
-        // fewer tiles than half the SMs (a tensor-parallel rank with 4 of the 32 heads): split EVERY tile's KV range so
-        // that the whole machine works on the launch
-        splits = fit_splits(slots / tiles);
-        if (splits >= 2) { n_split = tiles; n_full = 0; } else splits = 1;
-    }
+    const int tiles = n_qt * H * B;
+    int n_full, n_split, splits;
+    plan_split_tail(tiles, [&](int) { return n_kvb; }, n_full, n_split, splits);
     float* part_ws = nullptr;
     if (n_split > 0 && attn_part_workspace(stream, (size_t)n_split * splits * (128 * 128 + 256) * sizeof(float), &part_ws)) return -1;
     const int grid = n_full + n_split * splits;
     const float scale_log2 = scale * 1.4426950408889634f;
     const bool pdl = pdl_mode() != 0;
     LaunchScope ls(LK_ATTN, 4.0 * B * H * (double)Lq * L * 128, stream);
-    static unsigned long long attr_set = 0;  // bit per device
-    int dev = 0;
-    MMDP_CUDA(cudaGetDevice(&dev));
-    if (!(attr_set >> (dev & 63) & 1ull)) {
-        MMDP_CUDA(cudaFuncSetAttribute(attention_kernel<kBKV>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem));
-        attr_set |= 1ull << (dev & 63);
-    }
+    static unsigned long long attr_set = 0;
+    if (attn_smem_attr(attention_kernel<kBKV>, kAttnSmem, attr_set)) return -1;
     MMDP_CUDA(launch_ex(attention_kernel<kBKV>, dim3(grid), dim3(kAttnThreads), kAttnSmem, stream, pdl, false, tmQ, tmK, tmVt, out, H, L,
                         d_model, scale_log2, n_full, splits, part_ws, Lq));
     if (n_split > 0)
         MMDP_CUDA(launch_ex(attention_combine_kernel, dim3(n_split, 128), dim3(128), 0, stream, pdl, false, (const float*)part_ws, out, H, Lq,
                             d_model, scale_log2, n_full, splits));
+    return 0;
+}
+
+template <int kBKV>
+static int attention_packed_launch(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* vt, __nv_bfloat16* out,
+                                   const SegTable& segs, int H, int Lpad, float scale, cudaStream_t stream) {
+    constexpr int kAttnSmem = AttnCfg<kBKV>::kSmem;
+    if (segs.n <= 0 || segs.n > kMaxSegs || H <= 0) return set_error("attention_packed: %d sequences (1 to %d)", segs.n, kMaxSegs);
+    if (Lpad % 8) return set_error("attention_packed: Lpad must be a multiple of 8");
+    AttnSegs as{};
+    as.n = segs.n;
+    double work = 0;
+    for (int s = 0; s <= segs.n; ++s) {
+        as.start[s] = segs.start[s];
+        if (s == segs.n) break;
+        const int len = segs.start[s + 1] - segs.start[s];
+        if (len <= 0 || len > Lpad) return set_error("attention_packed: sequence %d has length %d (Lpad %d)", s, len, Lpad);
+        as.tile0[s + 1] = as.tile0[s] + (len + 127) / 128 * H;
+        work += 4.0 * H * (double)len * len * 128;
+    }
+    const int M = segs.start[segs.n], tiles = as.tile0[segs.n], d_model = H * 128;
+    CUtensorMap tmQ, tmK, tmVt;
+    if (make_tmap_2d_bf16(&tmQ, q, (uint64_t)M, (uint64_t)d_model, (uint64_t)d_model, 128, 64)) return -1;
+    if (make_tmap_2d_bf16(&tmK, k, (uint64_t)M, (uint64_t)d_model, (uint64_t)d_model, kBKV, 64)) return -1;
+    if (make_tmap_2d_bf16(&tmVt, vt, (uint64_t)segs.n * H * 128, (uint64_t)Lpad, (uint64_t)Lpad, 128, 64)) return -1;
+    auto kvb_of = [&](int t) {
+        int s = 0;
+        while (s + 1 < segs.n && t >= as.tile0[s + 1]) ++s;
+        return (segs.start[s + 1] - segs.start[s] + kBKV - 1) / kBKV;
+    };
+    int n_full, n_split, splits;
+    plan_split_tail(tiles, kvb_of, n_full, n_split, splits);
+    float* part_ws = nullptr;
+    if (n_split > 0 && attn_part_workspace(stream, (size_t)n_split * splits * (128 * 128 + 256) * sizeof(float), &part_ws)) return -1;
+    const int grid = n_full + n_split * splits;
+    const float scale_log2 = scale * 1.4426950408889634f;
+    const bool pdl = pdl_mode() != 0;
+    LaunchScope ls(LK_ATTN, work, stream);
+    static unsigned long long attr_set = 0;
+    if (attn_smem_attr(attention_packed_kernel<kBKV>, kAttnSmem, attr_set)) return -1;
+    MMDP_CUDA(launch_ex(attention_packed_kernel<kBKV>, dim3(grid), dim3(kAttnThreads), kAttnSmem, stream, pdl, false, tmQ, tmK, tmVt, out,
+                        H, d_model, scale_log2, n_full, splits, part_ws, as));
+    if (n_split > 0)
+        MMDP_CUDA(launch_ex(attention_packed_combine_kernel, dim3(n_split, 128), dim3(128), 0, stream, pdl, false, (const float*)part_ws,
+                            out, H, d_model, scale_log2, n_full, splits, as));
     return 0;
 }
 
@@ -339,6 +466,14 @@ int attention_fwd(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfl
     if (version == 7) return attention_launch<64>(q, k, vt, out, B, H, L, Lpad, scale, stream, Lq);
     if (version != 6) return set_error("attention: unknown kernel generation %d (6 or 7)", version);
     return attention_launch<128>(q, k, vt, out, B, H, L, Lpad, scale, stream, Lq);
+}
+
+int attention_packed_fwd(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* vt, __nv_bfloat16* out,
+                         const SegTable& segs, int H, int Lpad, float scale, cudaStream_t stream) {
+    const int version = opt(OPT_ATTN_VERSION);
+    if (version == 7) return attention_packed_launch<64>(q, k, vt, out, segs, H, Lpad, scale, stream);
+    if (version != 6) return set_error("attention: unknown kernel generation %d (6 or 7)", version);
+    return attention_packed_launch<128>(q, k, vt, out, segs, H, Lpad, scale, stream);
 }
 
 }  // namespace mmdp

@@ -238,10 +238,12 @@ int gemm_fp8(int epi, const uint8_t* A, int lda, const float* sa, const uint8_t*
             if (!C || (ldc % 8) || (N % kF8BN)) return set_error("gemm_fp8: swiglu needs N %% 128 == 0 (gate/up interleaved in 64-row blocks)");
             break;
         case EPI_QKVROPE:
+        case EPI_QKVROPE_PACKED:
             if (!qa) return set_error("gemm_fp8: qkv epilogue needs QkvRopeArgs");
             if (qa->d_model % 256 || N != 3 * qa->d_model || qa->d_model != qa->n_heads * 128)
                 return set_error("gemm_fp8: qkv epilogue needs head_dim 128, d_model %% 256 == 0, N == 3*d_model");
-            if (qa->pos_map ? (qa->Tq <= 0 || M % qa->Tq) : (!qa->chunked && (M % qa->L))) return set_error("gemm_fp8: qkv epilogue needs M == B*L (or B*Tq with a position map)");
+            if (epi == EPI_QKVROPE_PACKED ? !qa->seg_pos : (qa->pos_map ? (qa->Tq <= 0 || M % qa->Tq) : (!qa->chunked && (M % qa->L))))
+                return set_error("gemm_fp8: qkv epilogue needs M == B*L (or B*Tq with a position map, or a packed row map)");
             break;
         default:
             return set_error("gemm_fp8: unsupported epilogue %d", epi);
@@ -253,7 +255,7 @@ int gemm_fp8(int epi, const uint8_t* A, int lda, const float* sa, const uint8_t*
     if (qa) {
         p.q = qa->q; p.k = qa->k; p.vt = qa->vt; p.cos_tab = qa->cos_tab; p.sin_tab = qa->sin_tab;
         p.L = qa->L; p.Lpad = qa->Lpad; p.d_model = qa->d_model; p.n_heads = qa->n_heads;
-        p.pos_map = qa->pos_map; p.Tq = qa->Tq; p.row0 = qa->row0;
+        p.pos_map = qa->pos_map; p.Tq = qa->Tq; p.row0 = qa->row0; p.seg_pos = qa->seg_pos;
     }
     const Fp8Scales sc{sa, sw};
     const int tiles = ((M + kF8BM - 1) / kF8BM) * ((N + kF8BN - 1) / kF8BN);
@@ -265,6 +267,7 @@ int gemm_fp8(int epi, const uint8_t* A, int lda, const float* sa, const uint8_t*
         case EPI_PLAIN: return launch_gemm_fp8<EPI_PLAIN>(tmA, tmB, p, sc, grid, stream);
         case EPI_RESID: return launch_gemm_fp8<EPI_RESID>(tmA, tmB, p, sc, grid, stream);
         case EPI_SWIGLU: return launch_gemm_fp8<EPI_SWIGLU>(tmA, tmB, p, sc, grid, stream);
+        case EPI_QKVROPE_PACKED: return launch_gemm_fp8<EPI_QKVROPE_PACKED>(tmA, tmB, p, sc, grid, stream);
         default: return launch_gemm_fp8<EPI_QKVROPE>(tmA, tmB, p, sc, grid, stream);
     }
 }

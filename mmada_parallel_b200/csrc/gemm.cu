@@ -10,6 +10,7 @@
 //   EPI_RESID   : C = bf16( bf16(acc) + resid )                            (attn_out + residual :744/:953; ff_out :968/:970)
 //   EPI_QKVROPE : q,k = bf16( rope_fp32( bf16(acc) ) ), v^T = bf16(acc)    (q/k/v_proj :925-927 + RotaryEmbedding :402-435)
 //   EPI_SWIGLU  : C = bf16( bf16(silu(bf16(g))) * bf16(u) )                (ff_proj/up_proj/act/mul :962-967)
+//   EPI_QKVROPE_PACKED : EPI_QKVROPE over a packed variable-length batch (per-row sequence and position)
 #include "gemm_epilogue.cuh"
 
 #include <stdlib.h>
@@ -457,10 +458,12 @@ int gemm_bf16(int epi, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, 
             if (!C || (ldc % 8) || (N % 256)) return set_error("gemm: swiglu needs N % 256 == 0 (interleaved gate/up tiles)");
             break;
         case EPI_QKVROPE:
+        case EPI_QKVROPE_PACKED:
             if (!qa) return set_error("gemm: qkv epilogue needs QkvRopeArgs");
             if (qa->d_model % 256 || N != 3 * qa->d_model || qa->d_model != qa->n_heads * 128)
                 return set_error("gemm: qkv epilogue needs head_dim 128, d_model % 256 == 0, N == 3*d_model");
-            if (qa->pos_map ? (qa->Tq <= 0 || M % qa->Tq) : (!qa->chunked && (M % qa->L))) return set_error("gemm: qkv epilogue needs M == B*L (or B*Tq with a position map)");
+            if (epi == EPI_QKVROPE_PACKED ? !qa->seg_pos : (qa->pos_map ? (qa->Tq <= 0 || M % qa->Tq) : (!qa->chunked && (M % qa->L))))
+                return set_error("gemm: qkv epilogue needs M == B*L (or B*Tq with a position map, or a packed row map)");
             break;
         default:
             return set_error("gemm: unknown epilogue");
@@ -489,7 +492,7 @@ int gemm_bf16(int epi, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, 
     if (qa) {
         p.q = qa->q; p.k = qa->k; p.vt = qa->vt; p.cos_tab = qa->cos_tab; p.sin_tab = qa->sin_tab;
         p.L = qa->L; p.Lpad = qa->Lpad; p.d_model = qa->d_model; p.n_heads = qa->n_heads;
-        p.pos_map = qa->pos_map; p.Tq = qa->Tq; p.row0 = qa->row0;
+        p.pos_map = qa->pos_map; p.Tq = qa->Tq; p.row0 = qa->row0; p.seg_pos = qa->seg_pos;
     }
     // kernel selection: MMDP_GEMM_PAIR / mmdp_set_gemm_pair 0 (default) = one CTA per tile (with the split-K tail), 1 = CTA
     // pairs for M > 256, 2 = pairs only for M >= 4096 and N >= 8192
@@ -506,6 +509,7 @@ int gemm_bf16(int epi, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, 
             case EPI_F32: return launch_gemm_pair<EPI_F32, 256>(tmA, tmBh, p, pair_tiles, stream);
             case EPI_SWIGLU: return launch_gemm_pair<EPI_SWIGLU, 256>(tmA, tmBh, p, pair_tiles, stream);
             case EPI_QKVROPE: return launch_gemm_pair<EPI_QKVROPE, 256>(tmA, tmBh, p, pair_tiles, stream);
+            case EPI_QKVROPE_PACKED: return launch_gemm_pair<EPI_QKVROPE_PACKED, 256>(tmA, tmBh, p, pair_tiles, stream);
             default: return set_error("gemm: unknown epilogue");
         }
     }
@@ -533,6 +537,8 @@ int gemm_bf16(int epi, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, 
             return launch_gemm<EPI_SWIGLU, 256>(tmA, tmB, p, grid, stream);
         case EPI_QKVROPE:
             return launch_gemm<EPI_QKVROPE, 256>(tmA, tmB, p, grid, stream);
+        case EPI_QKVROPE_PACKED:
+            return launch_gemm<EPI_QKVROPE_PACKED, 256>(tmA, tmB, p, grid, stream);
         default:
             return set_error("gemm: unknown epilogue");
     }

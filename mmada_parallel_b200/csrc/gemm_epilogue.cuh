@@ -42,6 +42,9 @@ struct GemmParams {
     // tile order: group_m == 0 -> M-fastest over all m-tiles; > 0 -> M-fastest inside groups of group_m m-tiles, all n-tiles
     // of a group before the next group (keeps the group's A rows L2-resident while the weights stream)
     int group_m;
+    // EPI_QKVROPE_PACKED: (sequence, position) of every row of a packed variable-length batch; q / k stay at the row,
+    // v^T goes to vt[sequence][head][d][position]
+    const int2* seg_pos;
 };
 
 __host__ __device__ __forceinline__ void gemm_tile_coords(int tl, int num_m, int num_n, int group_m, int& m_blk, int& n_blk) {
@@ -116,10 +119,14 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
                 }
                 *reinterpret_cast<uint32_t*>(p.C + (size_t)row * p.ldc + col) = pack_bf16x2(o[0], o[1]);
             }
-        } else if constexpr (EPI == EPI_QKVROPE) {
+        } else if constexpr (EPI == EPI_QKVROPE || EPI == EPI_QKVROPE_PACKED) {
             const int region = n0 / p.d_model;  // 0 = Q, 1 = K, 2 = V (d_model % 256 == 0 is checked on the host)
             int b, pos;
-            if (p.pos_map) {
+            if constexpr (EPI == EPI_QKVROPE_PACKED) {
+                const int2 sp = p.seg_pos[row];
+                b = sp.x;
+                pos = sp.y;
+            } else if (p.pos_map) {
                 b = row / p.Tq;
                 pos = p.pos_map[row];
             } else {
@@ -278,7 +285,7 @@ __device__ __forceinline__ void sk_finish(const GemmParams& p, const float4* __r
             *reinterpret_cast<uint4*>(p.C + (size_t)row * p.ldc + col) =
                 make_uint4(pack_bf16x2(o[0], o[1]), pack_bf16x2(o[2], o[3]), pack_bf16x2(o[4], o[5]), pack_bf16x2(o[6], o[7]));
         }
-    } else if constexpr (EPI == EPI_QKVROPE) {
+    } else if constexpr (EPI == EPI_QKVROPE || EPI == EPI_QKVROPE_PACKED) {
         const int region = n0 / p.d_model;  // 0 = Q, 1 = K, 2 = V
         if (region < 2) {
             constexpr int G = 16;  // 2 heads x 8 column groups of the first half
@@ -291,7 +298,7 @@ __device__ __forceinline__ void sk_finish(const GemmParams& p, const float4* __r
                 const int col4[4] = {head * 32 + 2 * gg, head * 32 + 2 * gg + 1, head * 32 + 16 + 2 * gg, head * 32 + 16 + 2 * gg + 1};
                 float4 a[4];
                 sk_sum<BN, 4>(tile_ws, S, rit, col4, a);
-                const int pos = (row + p.row0) % p.L;
+                const int pos = EPI == EPI_QKVROPE_PACKED ? p.seg_pos[row].y : (row + p.row0) % p.L;
                 const float4* c4 = reinterpret_cast<const float4*>(p.cos_tab + (size_t)pos * 64 + 8 * gg);
                 const float4* s4 = reinterpret_cast<const float4*>(p.sin_tab + (size_t)pos * 64 + 8 * gg);
                 const float4 c0 = c4[0], c1 = c4[1], s0 = s4[0], s1 = s4[1];
@@ -321,7 +328,15 @@ __device__ __forceinline__ void sk_finish(const GemmParams& p, const float4* __r
                 const int col4[2] = {2 * g, 2 * g + 1};
                 float4 a[2];
                 sk_sum<BN, 2>(tile_ws, S, rit, col4, a);
-                const int b = (row + p.row0) / p.L, pos = (row + p.row0) - b * p.L;
+                int b, pos;
+                if constexpr (EPI == EPI_QKVROPE_PACKED) {
+                    const int2 sp = p.seg_pos[row];
+                    b = sp.x;
+                    pos = sp.y;
+                } else {
+                    b = (row + p.row0) / p.L;
+                    pos = (row + p.row0) - b * p.L;
+                }
                 const int n = n0 - 2 * p.d_model + 8 * g;
                 const int head = n >> 7, d0 = n & 127;
                 __nv_bfloat16* dst = p.vt + ((size_t)(b * p.n_heads + head) * 128 + d0) * p.Lpad + pos;

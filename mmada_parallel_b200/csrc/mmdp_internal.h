@@ -8,7 +8,17 @@
 
 namespace mmdp {
 
-enum Epilogue { EPI_PLAIN = 0, EPI_RESID = 1, EPI_QKVROPE = 2, EPI_SWIGLU = 3, EPI_F32 = 4 };
+// EPI_QKVROPE_PACKED: EPI_QKVROPE over a packed variable-length batch (QkvRopeArgs::seg_pos)
+enum Epilogue { EPI_PLAIN = 0, EPI_RESID = 1, EPI_QKVROPE = 2, EPI_SWIGLU = 3, EPI_F32 = 4, EPI_QKVROPE_PACKED = 5 };
+
+// Packed variable-length batch: sequence s occupies rows [start[s], start[s + 1]) of one packed row space; attention never
+// crosses from one sequence into another and positions restart at 0 in each. kMaxSegs bounds the sequences of one launch
+// (the table travels as a kernel parameter).
+static constexpr int kMaxSegs = 64;
+struct SegTable {
+    int n;
+    int start[kMaxSegs + 1];
+};
 
 int set_error(const char* fmt, ...);  // records the message for mmdp_last_error(), returns -1
 const char* last_error();
@@ -111,7 +121,12 @@ struct QkvRopeArgs {
     int Tq = 0;
     int chunked = 0;  // 1: the launch covers a row range of the [B*L] sequence (M need not be a multiple of L)
     int row0 = 0;  // GEMM row r is token row0 + r of the flattened [B*L] sequence (row-chunked tensor-parallel forward); q / k point at that row
+    const int2* seg_pos = nullptr;  // EPI_QKVROPE_PACKED: row r is token seg_pos[r].y of sequence seg_pos[r].x (q / k stay at row r,
+                                    // v^T goes to vt[seg][head][d][pos]); L is then the longest sequence
 };
+
+// device map of a packed batch: seg_pos[r] = (sequence, position) of packed row r, for the rows of `segs`
+int packed_row_map(const SegTable& segs, int2* seg_pos, cudaStream_t stream);
 
 // EPI_F32 only: push the fp32 partial rows to their owners' receive buffers instead of storing them to C (tensor parallel)
 struct GemmScatter {
@@ -142,6 +157,10 @@ void set_gemm_splitk_mode(int mode);
 // Lq > 0: q / out hold Lq query rows per batch row (a compact subset), k / vt the full L keys (token-cache forward)
 int attention_fwd(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* vt, __nv_bfloat16* out, int B,
                   int H, int L, int Lpad, float scale, cudaStream_t stream, int Lq = 0);
+// packed variable-length batch: q / k / out [segs.start[n], H * 128], vt [segs.n, H, 128, Lpad]; columns [L_s, Lpad) of
+// sequence s's V^T block must be finite zeros
+int attention_packed_fwd(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* vt, __nv_bfloat16* out,
+                         const SegTable& segs, int H, int Lpad, float scale, cudaStream_t stream);
 
 // err (nullable): device int, bit 0 is raised when an id is outside [0, vocab) (the kernel then reads row 0)
 int embed_rows(const int64_t* ids, const __nv_bfloat16* wte, __nv_bfloat16* x, int M, int d, int64_t vocab,

@@ -137,13 +137,32 @@ def denoise_step(st: DenoiseState, step: int, is_img: bool, k_transfer: int, noi
     on device-resident state. No host<->device synchronisation happens in here.
     `text_masks_left` is the number of masked text positions entering this step (known on the host without a read-back:
     total - sum of the transfer counts so far); at 0 the reference skips the whole text step INCLUDING its Gumbel draw
-    (`if text_masked_indices.sum() > 0`, :183), so no generator state is consumed here either."""
-    model, ids, V, n_text, seq_len = st.model, st.ids, st.model.vocab_rows, st.n_text, st.seq_len
+    (`if text_masked_indices.sum() > 0`, :183), so no generator state is consumed here either.
+    The forwards are issued here; the sampling halves (`text_sample`, `image_sample`) are shared with the packed batch loop
+    (generators/batch.py)."""
+    model, ids = st.model, st.ids
     # ---- conditional forward (:178): text rows x V, and the image rows x codebook window on image steps
     model.forward_rows(ids, rows_a=st.text_rows, out_a=st.text_logits, rows_b=st.pos if is_img else None,
                        col0_b=text_vocab_size, ncols_b=codebook_size, out_b=st.cond_vq if is_img else None,
                        **_window(model, st.win_both if is_img else st.win_text))
-    # ---- text step (:181-217), guarded like the reference's `.sum() > 0` (:183)
+    text_sample(st, step, k_transfer, noise, text_temperature, _trace, text_masks_left)
+    if not is_img:
+        return
+    # ---- unconditional forwards (:243-264) on the ids after the text step
+    for out_name, prefix in uncond_inputs(st, cfg_scale, cfg_img):
+        st.scratch_ids.copy_(ids)
+        if prefix is not None:
+            st.scratch_ids[:, : prefix.shape[1]] = prefix
+        model.forward_rows(st.scratch_ids, rows_b=st.pos, col0_b=text_vocab_size, ncols_b=codebook_size,
+                           out_b=getattr(st, out_name), **_window(model, st.win_img))
+    image_sample(st, step, noise, text_steps, temperature, cfg_scale, cfg_img, noise_schedule, text_vocab_size, codebook_size,
+                 _trace)
+
+
+def text_sample(st: DenoiseState, step: int, k_transfer: int, noise: "_Noise", text_temperature: float,
+                _trace: Optional[list] = None, text_masks_left: int = 1) -> None:
+    """Text step (:181-217) on the conditional text logits in `st.text_logits`, guarded like the reference's `.sum() > 0` (:183)."""
+    ids, V, n_text = st.ids, st.model.vocab_rows, st.n_text
     if text_masks_left > 0:
         un = noise.rand((1, n_text, V))[0] if text_temperature != 0 else None
         check(lib.mmdp_text_step(ptr(st.text_logits), None, V, n_text, V, 0.0, ptr(un), V, float(text_temperature),
@@ -151,25 +170,30 @@ def denoise_step(st: DenoiseState, step: int, is_img: bool, k_transfer: int, noi
                                  stream_ptr()))
     if _trace is not None:
         _trace.append({"step": step, "ids_after_text": ids[0].clone()})
-    if not is_img:
-        return
-    # ---- image step (:220-344)
+
+
+def uncond_inputs(st: DenoiseState, cfg_scale: float, cfg_img: float) -> list:
+    """The unconditional forwards of an image step (:243-264), in the reference's order: [(name of the DenoiseState buffer that
+    receives the image-row logits, prefix ids [1, n] that replace the start of the sequence, or None)]. Each runs on the ids
+    after the text step with the prefix written over them; its length is the sequence's."""
+    if not st.use_uncond:
+        return []
+    out = []
+    if cfg_scale != 0.0:
+        out.append(("unc_t_vq", st.unc_t_ids))
+    if cfg_img != 0.0:
+        out.append(("unc_i_vq", st.unc_i_ids))
+    return out
+
+
+def image_sample(st: DenoiseState, step: int, noise: "_Noise", text_steps: int, temperature: float, cfg_scale: float,
+                 cfg_img: float, noise_schedule, text_vocab_size: int, codebook_size: int, _trace: Optional[list] = None) -> None:
+    """Image step (:220-344) on the logits in `st.cond_vq` and the unconditional buffers named by `uncond_inputs`."""
+    ids, seq_len = st.ids, st.seq_len
     ua = ub = None
     if st.use_uncond:
-        if cfg_scale != 0.0:
-            st.scratch_ids.copy_(ids)
-            if st.unc_t_ids is not None:
-                st.scratch_ids[:, : st.unc_t_ids.shape[1]] = st.unc_t_ids
-            model.forward_rows(st.scratch_ids, rows_b=st.pos, col0_b=text_vocab_size, ncols_b=codebook_size, out_b=st.unc_t_vq,
-                               **_window(model, st.win_img))
-            ua = st.unc_t_vq
-        if cfg_img != 0.0:
-            st.scratch_ids.copy_(ids)
-            if st.unc_i_ids is not None:
-                st.scratch_ids[:, : st.unc_i_ids.shape[1]] = st.unc_i_ids
-            model.forward_rows(st.scratch_ids, rows_b=st.pos, col0_b=text_vocab_size, ncols_b=codebook_size, out_b=st.unc_i_vq,
-                               **_window(model, st.win_img))
-            ub = st.unc_i_vq
+        ua = st.unc_t_vq if cfg_scale != 0.0 else None
+        ub = st.unc_i_vq if cfg_img != 0.0 else None
     elif st.zeros_vq is not None:
         # no uncond inputs: the reference mixes against zeros (:277-278)
         ua = st.zeros_vq if cfg_scale != 0.0 else None
@@ -232,13 +256,7 @@ def generate_ti2ti(
 ):
     """Joint text+image mask-predict generation. Arguments, defaults, side effects (input_ids is not modified) and
     return value `(List[int] image VQ tokens, str | List[int] text)` are those of the reference function."""
-    if remasking != "low_confidence":
-        # 'random' requests int64 uniform noise in the reference and raises there too (:195-197)
-        raise NotImplementedError(remasking)
-    if not hasattr(model, "forward_rows"):
-        raise TypeError("generate_ti2ti needs a mmada_parallel_b200.model.LLaDAForMultiModalGeneration (H100-native) model")
-    if input_ids.shape[0] != 1:
-        raise ValueError("the image path of generate_ti2ti is single-sample (reference :224/:340 read batch row 0 only)")
+    check_request(model, input_ids, remasking)
     ids_host = input_ids.detach().to("cpu", torch.int64)
     total_image_len = seq_len + seq_len // newline_every
     print(f"Interleaved generation: {text_steps} total steps")
@@ -254,16 +272,33 @@ def generate_ti2ti(
     final = ids[0].cpu()
     if hasattr(model, "raise_device_errors"):
         model.raise_device_errors()   # e.g. a token id outside the vocabulary: IndexError, like nn.Embedding in the reference
-    text_tokens = [t for t in final[text_start:text_end].tolist() if t != MASK_TOKEN]
+    image_tokens, generated_text, n_text_tokens = extract_results(st, final, tokenizer, text_vocab_size, codebook_size)
+    print("Interleaved generation complete.")
+    print(f"  - Generated text: {n_text_tokens} tokens")
+    print(f"  - Generated image: {len(image_tokens)} VQ tokens (range [0, {codebook_size}))")
+    return image_tokens, generated_text
+
+
+def check_request(model, input_ids, remasking) -> None:
+    """The argument checks generate_ti2ti makes before it builds its state, in its order."""
+    if remasking != "low_confidence":
+        # 'random' requests int64 uniform noise in the reference and raises there too (:195-197)
+        raise NotImplementedError(remasking)
+    if not hasattr(model, "forward_rows"):
+        raise TypeError("generate_ti2ti needs a mmada_parallel_b200.model.LLaDAForMultiModalGeneration (H100-native) model")
+    if input_ids.shape[0] != 1:
+        raise ValueError("the image path of generate_ti2ti is single-sample (reference :224/:340 read batch row 0 only)")
+
+
+def extract_results(st: DenoiseState, final: torch.Tensor, tokenizer, text_vocab_size: int, codebook_size: int):
+    """(:346-368) The image VQ tokens and the text of the final id row `final` (host). Image tokens still masked are drawn
+    from the GLOBAL CPU RNG like the reference (:362). Returns (image tokens, text, number of text tokens)."""
+    text_tokens = [t for t in final[st.text_start:st.text_end].tolist() if t != MASK_TOKEN]
     generated_text = tokenizer.decode(text_tokens, skip_special_tokens=True) if tokenizer is not None else text_tokens
     image_tokens: List[int] = []
     for t in final[torch.tensor(st.pos_list)].tolist():
         if t != MASK_TOKEN:
             image_tokens.append(max(0, min(t - text_vocab_size, codebook_size - 1)))
         else:
-            # still masked -> sampled from the GLOBAL CPU RNG exactly like the reference (:362)
             image_tokens.append(int(torch.randint(0, codebook_size, (1,)).item()))
-    print("Interleaved generation complete.")
-    print(f"  - Generated text: {len(text_tokens)} tokens")
-    print(f"  - Generated image: {len(image_tokens)} VQ tokens (range [0, {codebook_size}))")
-    return image_tokens, generated_text
+    return image_tokens, generated_text, len(text_tokens)

@@ -306,3 +306,30 @@ class LLaDAForMultiModalGeneration:
         check(lib.mmdp_model_forward_window(self._h, ptr(ids), B, L, ptr(rows_a), n_a, ptr(out_a) if n_a else None,
                                             ptr(rows_b), n_b, col0_b, ncols_b, ptr(out_b) if n_b else None, lo, hi, stream_ptr()))
         return (out_a if n_a else None), (out_b if n_b else None)
+
+    def forward_rows_packed(self, ids_packed: torch.Tensor, seq_lens, rows_a: Optional[torch.Tensor] = None,
+                            rows_b: Optional[torch.Tensor] = None, col0_b: int = 0, ncols_b: int = 0,
+                            out_a: Optional[torch.Tensor] = None, out_b: Optional[torch.Tensor] = None):
+        """One forward over a packed batch of several sequences of different lengths: ids_packed [sum(seq_lens)] (cuda int64) holds
+        the sequences end to end. Each sequence is computed as if it were alone (attention stays inside it, positions restart at
+        0), so its logits equal those of its own `forward_rows`. rows_* are int32 packed row indices (offset of the sequence +
+        position). Returns (logits_a [n_a, V] or None, logits_b [n_b, ncols_b] or None), like `forward_rows`.
+        At most `max_batch` sequences, each at most `max_seq_len` long (ValueError otherwise)."""
+        lens = [int(x) for x in seq_lens]
+        if not lens or len(lens) > self.max_batch:
+            raise ValueError(f"a packed forward takes 1 to max_batch={self.max_batch} sequences, got {len(lens)}")
+        if min(lens) < 1 or max(lens) > self.max_seq_len:
+            raise ValueError(f"packed sequence lengths must lie in [1, max_seq_len={self.max_seq_len}], got {lens}")
+        if ids_packed.numel() != sum(lens):
+            raise ValueError(f"ids_packed holds {ids_packed.numel()} tokens, the sequence lengths add up to {sum(lens)}")
+        ids = ids_packed.to(device=self.device, dtype=torch.int64).contiguous()
+        n_a = 0 if rows_a is None else rows_a.numel()
+        n_b = 0 if rows_b is None else rows_b.numel()
+        if n_a and out_a is None:
+            out_a = torch.empty((n_a, self.vocab_rows), dtype=torch.bfloat16, device=self.device)
+        if n_b and out_b is None:
+            out_b = torch.empty((n_b, ncols_b), dtype=torch.bfloat16, device=self.device)
+        c_lens = (C.c_int32 * len(lens))(*lens)
+        check(lib.mmdp_model_forward_packed(self._h, ptr(ids), len(lens), c_lens, ptr(rows_a), n_a, ptr(out_a) if n_a else None,
+                                            ptr(rows_b), n_b, col0_b, ncols_b, ptr(out_b) if n_b else None, stream_ptr()))
+        return (out_a if n_a else None), (out_b if n_b else None)
