@@ -161,10 +161,12 @@ int conv_tf32(const float* A, int lda, long long a_rows, const float* W, int M, 
     CUtensorMap tmA, tmW;
     if (make_tmap_2d(&tmA, A, 4, (uint64_t)a_rows, (uint64_t)K, (uint64_t)lda, CBM, CBK)) return -1;
     if (make_tmap_2d(&tmW, W, 4, (uint64_t)T * N, (uint64_t)K, (uint64_t)K, CBN, CBK)) return -1;
-    static bool attr_set = false;
-    if (!attr_set) {
+    static unsigned long long attr_set = 0;  // bit per device: the attribute is a property of each device's module
+    int dev = 0;
+    MMDP_CUDA(cudaGetDevice(&dev));
+    if (!(attr_set >> (dev & 63) & 1ull)) {
         MMDP_CUDA(cudaFuncSetAttribute(conv_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kConvSmem));
-        attr_set = true;
+        attr_set |= 1ull << (dev & 63);
     }
     const int num_tiles = ((M + CBM - 1) / CBM) * ((N + CBN - 1) / CBN);
     const int grid = num_tiles < num_sms() ? num_tiles : num_sms();
@@ -179,12 +181,23 @@ int conv_tf32(const float* A, int lda, long long a_rows, const float* W, int M, 
 // ------------------------------------------------------------------------------------------------
 // GroupNorm(32 groups) statistics over the interior pixels of padded NHWC images. grid (chunks, B); thread layout:
 // TC = min(C, 256) lanes along channels (coalesced), 256/TC lanes along pixels; fp64 accumulation across CTAs.
+//
+// The sums are taken of x - p, with p the group's pivot: its first channel at the first interior pixel (gn_pivot). Plain
+// sums of x and x^2 give var = E[x^2] - mean^2, which cancels catastrophically once |mean| >> std (the fp32 per-thread sums
+// lose ~|mean/std|^2 * 2^-24 of the variance: 0.1 % at mean/std = 1000); a pivot drawn from the group itself leaves
+// |mean - p| of the order of the group's spread, so the shifted moments keep the variance to a few fp32 ulps at any offset.
+__device__ __forceinline__ float gn_pivot(const float* __restrict__ xb, int C, int Wp, int g) {
+    return xb[(size_t)(Wp + 1) * C + g * (C / 32)];
+}
+
 __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__ x, int C, int H, int W, double* __restrict__ stats) {
-    // per-(image, group) sum and sum of squares of the interior pixels. A thread owns four consecutive channels (one float4) and
-    // walks the CTA's pixel chunk with 256 / (C/4) pixel lanes, four independent loads in flight (the first version - one
-    // scalar load per thread and iteration, 256 CTAs - ran at 0.5 TB/s on the 134 MB full-resolution tensors: latency-bound)
+    // per-(image, group) sum and sum of squares of x - pivot over the interior pixels. A thread owns four consecutive channels
+    // (one float4) and walks the CTA's pixel chunk with 256 / (C/4) pixel lanes, four independent loads in flight (the first
+    // version - one scalar load per thread and iteration, 256 CTAs - ran at 0.5 TB/s on the 134 MB full-resolution tensors:
+    // latency-bound)
     const int b = blockIdx.y, Wp = W + 2, cpg = C / 32, C4 = C / 4;
-    const float4* xb = reinterpret_cast<const float4*>(x + (size_t)b * (H + 2) * Wp * C);
+    const float* xf = x + (size_t)b * (H + 2) * Wp * C;
+    const float4* xb = reinterpret_cast<const float4*>(xf);
     const int TC = C4 < 256 ? C4 : 256, PP = 256 / TC;
     const int cl = threadIdx.x % TC, pl = threadIdx.x / TC;
     const long long npix = (long long)H * W;
@@ -196,7 +209,9 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__
     __syncthreads();
     if (pl < PP) {
         for (int c4 = cl; c4 < C4; c4 += TC) {
-            float s[4] = {0.f, 0.f, 0.f, 0.f}, q[4] = {0.f, 0.f, 0.f, 0.f};
+            float s[4] = {0.f, 0.f, 0.f, 0.f}, q[4] = {0.f, 0.f, 0.f, 0.f}, pv[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) pv[k] = gn_pivot(xf, C, Wp, (c4 * 4 + k) / cpg);
             for (long long pp = p0 + pl; pp < p1; pp += 4LL * PP) {
                 float4 v[4];
 #pragma unroll
@@ -206,14 +221,14 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__
                         const int y = (int)(pt / W), xx = (int)(pt - (long long)y * W);
                         v[t] = xb[((size_t)(y + 1) * Wp + xx + 1) * C4 + c4];
                     } else {
-                        v[t] = make_float4(0.f, 0.f, 0.f, 0.f);
+                        v[t] = make_float4(pv[0], pv[1], pv[2], pv[3]);  // contributes x - pivot = 0
                     }
                 }
 #pragma unroll
                 for (int t = 0; t < 4; ++t) {
-                    s[0] += v[t].x; s[1] += v[t].y; s[2] += v[t].z; s[3] += v[t].w;
-                    q[0] = fmaf(v[t].x, v[t].x, q[0]); q[1] = fmaf(v[t].y, v[t].y, q[1]);
-                    q[2] = fmaf(v[t].z, v[t].z, q[2]); q[3] = fmaf(v[t].w, v[t].w, q[3]);
+                    const float d[4] = {v[t].x - pv[0], v[t].y - pv[1], v[t].z - pv[2], v[t].w - pv[3]};
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) { s[k] += d[k]; q[k] = fmaf(d[k], d[k], q[k]); }
                 }
             }
 #pragma unroll
@@ -240,10 +255,11 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const float* __restrict__
     const int b = blockIdx.y, yy = blockIdx.x, Wp = W + 2, Hp = H + 2, cpg = C / 32, C4 = C / 4;
     __shared__ float s_mean[32], s_rstd[32];
     if (threadIdx.x < 32) {
+        // moments of x - pivot (gn_stats_kernel); var is clamped at 0 so that rounding can never make var + eps negative
         const double cnt = (double)H * W * cpg;
-        const double mean = stats[((size_t)b * 32 + threadIdx.x) * 2] / cnt;
-        const double var = stats[((size_t)b * 32 + threadIdx.x) * 2 + 1] / cnt - mean * mean;
-        s_mean[threadIdx.x] = (float)mean;
+        const double m1 = stats[((size_t)b * 32 + threadIdx.x) * 2] / cnt;
+        const double var = fmax(stats[((size_t)b * 32 + threadIdx.x) * 2 + 1] / cnt - m1 * m1, 0.0);
+        s_mean[threadIdx.x] = (float)((double)gn_pivot(x + (size_t)b * Hp * Wp * C, C, Wp, threadIdx.x) + m1);
         s_rstd[threadIdx.x] = (float)(1.0 / sqrt(var + (double)eps));
     }
     __syncthreads();

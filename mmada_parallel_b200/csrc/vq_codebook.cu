@@ -142,10 +142,12 @@ int vq_nearest(const float* z, const float* cb, int B, int C, int h, int w, int 
     if (Nl > 0x7fffffffLL) return set_error("vq_nearest: too many latent vectors");
     const int N = (int)Nl, hw = h * w;
     const int smem = (C * kNnVec + kNnCodes * (C + 1)) * 4;
-    static bool attr_set = false;
-    if (!attr_set) {
+    static unsigned long long attr_set = 0;  // bit per device: the attribute is a property of each device's module
+    int dev = 0;
+    MMDP_CUDA(cudaGetDevice(&dev));
+    if (!(attr_set >> (dev & 63) & 1ull)) {
         MMDP_CUDA(cudaFuncSetAttribute(vq_nearest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (256 * kNnVec + kNnCodes * 257) * 4));
-        attr_set = true;
+        attr_set |= 1ull << (dev & 63);
     }
     // split the codebook so that about two CTAs per SM run
     const int gx = (N + kNnVec - 1) / kNnVec;

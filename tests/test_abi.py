@@ -62,3 +62,21 @@ def test_product_never_imports_oracle():
                 src = open(os.path.join(dp, f)).read()
                 assert not re.search(r"^\s*(from|import)\s+oracle", src, re.M), f"{f} imports oracle"
                 assert "/root/reference" not in src
+
+
+def test_testing_hooks_exported_and_fail_without_gpu():
+    """Every hook of include/mmdp_testing.h is exported, kept out of the product table, and errors (not crashes) without a
+    device."""
+    from mmada_parallel_b200 import _lib
+    from test_gpu_vq_ops import HOOKS, declared_testing_symbols, hooks
+    names = declared_testing_symbols()
+    assert len(names) == 11 and sorted(HOOKS) == names
+    lib = hooks()
+    for n in names:
+        assert n not in _lib.SIGNATURES
+    if torch.cuda.is_available():
+        return
+    for n, args in HOOKS.items():
+        zeros = [0.0 if a is C.c_float else None if a is C.c_void_p else 1 for a in args]
+        assert getattr(lib, n)(*zeros) == -1, n
+        assert b"no CUDA device" in _lib.lib.mmdp_last_error(), n
