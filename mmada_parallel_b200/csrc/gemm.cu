@@ -1,8 +1,11 @@
 // Persistent warp-specialised bf16 GEMM for sm_90a:  C[M,N] = A[M,K] · W[N,K]^T  (fp32 accumulate in registers)
 //
-//   warpgroup 0    : TMA producer  (one elected thread: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx)
-//   warpgroups 1,2 : MMA + epilogue (wgmma m64nBNk16, one 64-row half of the 128 x BN tile each; the fused epilogue runs
-//                    on the register fragments while the producer already fills the ring with the next tile's k-blocks)
+//   warpgroup 0    : TMA producer  (warp 0, one elected thread: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier
+//                    complete_tx) and, in warps 1-3, the fused epilogue of the previous tile (staged epilogues)
+//   warpgroups 1,2 : MMA (wgmma m64nBNk16, one 64-row half of the 128 x BN tile each). After the last k-block they write the
+//                    tile as bf16 into a staging tile in shared memory and go straight on to the next tile's k-blocks; the
+//                    epilogue warps apply the fused epilogue from there with 16-byte loads and stores. The fp32 partials
+//                    (EPI_F32) and the split-K tail keep the epilogue on the register fragments.
 //
 // Every nn.Linear of the reference block (MMaDA-Parallel-A/model/modeling_llada.py:925-927, :744, :962, :968, :1402)
 // maps to one launch of this kernel with a fused epilogue that reproduces the reference's bf16 rounding points:
@@ -24,26 +27,156 @@ namespace mmdp {
 static constexpr int BM = 128, BK = 64;
 static constexpr int kABytes = BM * BK * 2;  // 16 KB
 static constexpr int kGemmThreads = 384;
+static constexpr int kStagedEpiThreads = 96;  // warps 1-3 of the producer warpgroup run the staged epilogue
 // The N tile width is a template parameter: 256 (default; required by the QKV/SwiGLU epilogues) or 192. The K loop and
 // therefore the fp32 accumulation order of every output element is identical for both, so results do not depend on
 // the tile width; the host picks the width that minimises (waves x width) for the problem (wave quantisation on the SMs).
-template <int BN> struct GemmCfg {
+// kStaged: the tile leaves the MMA warps as bf16 through a staging tile in shared memory (128 rows of BN bf16, rows padded by
+// 16 bytes) that the epilogue warps drain while the MMA warps run the next tile; the staging tile takes one ring stage.
+template <int BN, bool kStaged> struct GemmCfg {
     static constexpr int kBBytes = BN * BK * 2;
     static constexpr int kStageBytes = kABytes + kBBytes;
-    static constexpr int kStages = (BN == 256) ? 4 : 5;  // 192 / 200 KB of the 227 KB an H100 block may use
-    static constexpr int kSmem = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+    static constexpr int kStages = (BN == 256 ? 4 : 5) - (kStaged ? 1 : 0);  // ring: 192 / 200 KB, staged 144 / 160 KB
+    static constexpr int kStagingStride = BN * 2 + 16;
+    static constexpr int kStagingBytes = kStaged ? BM * kStagingStride : 0;  // 66 / 50 KB
+    static constexpr int kSmem = kStages * kStageBytes + kStagingBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+    static_assert(kSmem <= 227 * 1024, "an H100 block may use 227 KB of shared memory");
 };
+// every epilogue except the fp32 partials rounds the accumulator to bf16 first, so a bf16 staging tile is exact
+template <int EPI> constexpr bool gemm_staged() { return EPI != EPI_F32; }
+
+// MMA warps: this thread's fragment (gemm_epilogue_tile's mapping) into the staging tile as bf16 pairs. Banks: a warp's store
+// covers 8 rows x 4 consecutive words; the row stride is BN / 2 + 4 words = 4 (mod 32), so the 32 words fall in 32 banks.
+template <int BN>
+__device__ __forceinline__ void stage_tile(uint8_t* stg, const float (&acc)[BN / 2], int rit0, int c0) {
+    constexpr int kStride = GemmCfg<BN, true>::kStagingStride;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j)
+            *reinterpret_cast<uint32_t*>(stg + (rit0 + 8 * h) * kStride + (8 * j + c0) * 2) = pack_bf16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+}
+
+__device__ __forceinline__ void bf16x8_to_float(uint4 x, float (&f)[8]) {
+    const uint32_t xs[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) { f[2 * i] = bf16_lo(xs[i]); f[2 * i + 1] = bf16_hi(xs[i]); }
+}
+
+// V^T of a staged QKV tile: items are 8 rows x 8 columns. When the 8 rows are 8 consecutive positions of one sequence starting
+// at a multiple of 8, the block is transposed in registers and each column (one d of V^T) is one 16-byte store; otherwise
+// (a sequence boundary inside the 8 rows, a position map, rows past M) every row goes through epi_row8's element stores.
+template <int EPI, int BN>
+__device__ __forceinline__ void staged_vt(const GemmParams& p, const uint8_t* stg, int m_blk, int n_blk, int etid) {
+    constexpr int kStride = GemmCfg<BN, true>::kStagingStride;
+    constexpr int CG = BN / 8;
+    const bool aligned = (p.Lpad & 7) == 0 && (reinterpret_cast<uintptr_t>(p.vt) & 15) == 0;
+    for (int idx = etid; idx < 16 * CG; idx += kStagedEpiThreads) {
+        const int rg = idx / CG, cg = idx - rg * CG;
+        const int r0 = m_blk * 128 + 8 * rg;
+        if (r0 >= p.M) continue;
+        uint4 x[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) x[i] = *reinterpret_cast<const uint4*>(stg + (8 * rg + i) * kStride + 16 * cg);
+        int b0, pos0;
+        qkv_row_coords<EPI>(p, r0, b0, pos0);
+        bool vec = aligned && r0 + 7 < p.M && (pos0 & 7) == 0;
+        for (int i = 1; i < 8 && vec; ++i) {
+            int b, pos;
+            qkv_row_coords<EPI>(p, r0 + i, b, pos);
+            vec = b == b0 && pos == pos0 + i;
+        }
+        if (vec) {
+            const int n = n_blk * BN - 2 * p.d_model + 8 * cg;
+            const int head = n >> 7, d0 = n & 127;
+            __nv_bfloat16* dst = p.vt + ((size_t)(b0 * p.n_heads + head) * 128 + d0) * p.Lpad + pos0;
+#pragma unroll
+            for (int c = 0; c < 8; ++c) {
+                uint32_t o[4];
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const uint4 a = x[2 * k], b = x[2 * k + 1];
+                    const uint32_t wa = (c >> 1) == 0 ? a.x : (c >> 1) == 1 ? a.y : (c >> 1) == 2 ? a.z : a.w;
+                    const uint32_t wb = (c >> 1) == 0 ? b.x : (c >> 1) == 1 ? b.y : (c >> 1) == 2 ? b.z : b.w;
+                    o[k] = __byte_perm(wa, wb, (c & 1) ? 0x7632 : 0x5410);  // column c of rows 2k (low half) and 2k + 1
+                }
+                *reinterpret_cast<uint4*>(dst + (size_t)c * p.Lpad) = make_uint4(o[0], o[1], o[2], o[3]);
+            }
+        } else {
+            const uint4 zero = make_uint4(0, 0, 0, 0);
+#pragma unroll 1
+            for (int i = 0; i < 8; ++i) {
+                if (r0 + i >= p.M) break;
+                float v[8];
+                bf16x8_to_float(x[i], v);
+                epi_row8<EPI, BN>(p, r0 + i, n_blk, 8 * cg, v, v, zero);
+            }
+        }
+    }
+}
+
+// Epilogue warps: the fused epilogue of one staged tile. Items are (row, 8-column group) as in the split-K finishing pass;
+// consecutive threads take consecutive groups of a row, so a warp reads a row's 16-byte chunks (512 contiguous bytes: no
+// bank conflict) and its global loads and stores are whole 16-byte pieces of one or two rows. Plain and residual items run
+// U at a time with all their loads issued before the first store (C may be the residual: the compiler cannot reorder them).
+template <int EPI, int BN>
+__device__ __forceinline__ void staged_epilogue(const GemmParams& p, const uint8_t* stg, int m_blk, int n_blk, int etid) {
+    constexpr int kStride = GemmCfg<BN, true>::kStagingStride;
+    if constexpr (EPI == EPI_QKVROPE || EPI == EPI_QKVROPE_PACKED) {
+        if (n_blk * BN >= 2 * p.d_model) {
+            staged_vt<EPI, BN>(p, stg, m_blk, n_blk, etid);
+            return;
+        }
+    }
+    constexpr bool kPair = EPI == EPI_SWIGLU || EPI == EPI_QKVROPE || EPI == EPI_QKVROPE_PACKED;
+    constexpr int G = kPair ? 16 : BN / 8;
+    constexpr int kItems = BM * G;
+    constexpr int U = kPair ? 1 : 4;
+    for (int i0 = etid; i0 < kItems; i0 += U * kStagedEpiThreads) {
+        uint4 xv[U], xw[U], rv[U];
+        int row[U], tc[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            const int idx = i0 + u * kStagedEpiThreads;
+            const int rit = idx / G, g = idx - rit * G;
+            // SwiGLU g -> gate columns 8g, up +128; rotary g = (head, gg) -> 128 head + 8 gg, partner +64
+            tc[u] = EPI == EPI_SWIGLU ? 8 * g : (kPair ? (g >> 3) * 128 + 8 * (g & 7) : 8 * g);
+            row[u] = (idx < kItems && m_blk * BM + rit < p.M) ? m_blk * BM + rit : -1;
+            rv[u] = make_uint4(0, 0, 0, 0);
+            if (row[u] < 0) continue;
+            xv[u] = *reinterpret_cast<const uint4*>(stg + rit * kStride + tc[u] * 2);
+            if constexpr (kPair) xw[u] = *reinterpret_cast<const uint4*>(stg + rit * kStride + (tc[u] + (EPI == EPI_SWIGLU ? 128 : 64)) * 2);
+            if constexpr (EPI == EPI_RESID) {
+                if (n_blk * BN + tc[u] < p.N) rv[u] = *reinterpret_cast<const uint4*>(p.resid + (size_t)row[u] * p.ldr + n_blk * BN + tc[u]);
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            if (row[u] < 0) continue;
+            float v[8], w[8];
+            bf16x8_to_float(xv[u], v);
+            if constexpr (kPair) bf16x8_to_float(xw[u], w);
+            epi_row8<EPI, BN>(p, row[u], n_blk, tc[u], v, kPair ? w : v, rv[u]);
+        }
+    }
+}
 
 template <int EPI, int BN>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
-    constexpr int kStages = GemmCfg<BN>::kStages;
-    constexpr int kStageBytes = GemmCfg<BN>::kStageBytes;
+    constexpr bool kStaged = gemm_staged<EPI>();
+    constexpr int kStages = GemmCfg<BN, kStaged>::kStages;
+    constexpr int kStageBytes = GemmCfg<BN, kStaged>::kStageBytes;
     static_assert(EPI == EPI_PLAIN || EPI == EPI_RESID || EPI == EPI_F32 || BN == 256, "fused QKV / SwiGLU epilogues need 256-wide tiles");
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
+    uint8_t* staging = smem + kStages * kStageBytes;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + GemmCfg<BN, kStaged>::kStagingBytes);
     uint64_t* empty_bar = full_bar + kStages;
+    // staged epilogue: "staged" completes when the MMA warps have written a tile into the staging tile, "drained" when the
+    // epilogue warps have read it; the k-th full tile of this CTA completes phase k of each
+    uint64_t* staged_bar = empty_bar + kStages;
+    uint64_t* drained_bar = staged_bar + 1;
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -55,6 +188,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int s = 0; s < kStages; ++s) {
             mbar_init(&full_bar[s], 1);
             mbar_init(&empty_bar[s], 8);  // one arrive per MMA warp
+        }
+        if constexpr (kStaged) {
+            mbar_init(staged_bar, 256);                 // every MMA thread, after its stores
+            mbar_init(drained_bar, kStagedEpiThreads);  // every epilogue thread, after its loads
         }
         fence_barrier_init();
     }
@@ -78,8 +215,22 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const int unit_kb1 = (unit_kb0 + p.sk_kb_per < num_k) ? unit_kb0 + p.sk_kb_per : num_k;
 
     if (wg == 0) {
-        // ===================== TMA producer =====================
-        setmaxnreg_dec<40>();
+        // ===================== TMA producer (warp 0) and staged epilogue (warps 1-3) =====================
+        // 56 / 224 / 224 registers per thread: 64 512 of the 65 536 for 384 threads
+        setmaxnreg_dec<kStaged ? 56 : 40>();
+        if constexpr (kStaged) {
+            if (warp > 0) {
+                const int etid = threadIdx.x - 32;
+                uint32_t it = 0;
+                for (int tile = blockIdx.x; tile < full_tiles; tile += gridDim.x, ++it) {  // the split-K unit never stages
+                    int m_blk, n_blk;
+                    gemm_tile_coords(tile, num_m, num_n, p.group_m, m_blk, n_blk);
+                    mbar_wait(staged_bar, it & 1);
+                    staged_epilogue<EPI, BN>(p, staging, m_blk, n_blk, etid);
+                    mbar_arrive(drained_bar);
+                }
+            }
+        }
         if (warp == 0 && elect_one_sync()) {
             int s = 0;
             uint32_t ph = 0;
@@ -107,13 +258,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         __syncwarp();
     } else {
         // ===================== MMA + epilogue (warpgroups 1 and 2: tile rows [64 (wg-1), 64 wg)) =====================
-        setmaxnreg_inc<232>();
+        setmaxnreg_inc<kStaged ? 224 : 232>();
         const int half = wg - 1;
         const int rit0 = half * 64 + (warp & 3) * 16 + (lane >> 2);  // tile row of acc[4j + 0..1]; acc[4j + 2..3] is 8 rows below
         const int c0 = 2 * (lane & 3);
         float acc[BN / 2];
         int s = 0;
         uint32_t ph = 0;
+        uint32_t it = 0;  // full tiles staged so far
         for (int tile = blockIdx.x; tile < full_tiles + (has_unit ? 1 : 0) * gridDim.x; tile += gridDim.x) {
             const bool is_unit = tile >= full_tiles;
             const int tl = is_unit ? unit_tile : tile;
@@ -174,7 +326,16 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 }
                 break;
             }
-            gemm_epilogue_tile<EPI, BN>(p, acc, m_blk, n_blk, rit0, c0);
+            if constexpr (kStaged) {
+                // the previous tile has left the staging tile a whole main loop ago; the epilogue warps apply the fused
+                // epilogue while this warpgroup runs the next tile's k-blocks
+                mbar_wait(drained_bar, (it & 1) ^ 1);
+                stage_tile<BN>(staging, acc, rit0, c0);
+                mbar_arrive(staged_bar);
+                ++it;
+            } else {
+                gemm_epilogue_tile<EPI, BN>(p, acc, m_blk, n_blk, rit0, c0);
+            }
         }
         if constexpr (EPI == EPI_F32) {
             if (p.scat_R > 0) __threadfence_system();  // the pushed rows are visible to their owners before this grid completes
@@ -191,8 +352,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 template <int EPI, int BN>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kGemmThreads, 1)
 gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBh, const GemmParams p) {
-    constexpr int kStages = GemmCfg<BN>::kStages;
-    constexpr int kStageBytes = GemmCfg<BN>::kStageBytes;
+    constexpr int kStages = GemmCfg<BN, false>::kStages;
+    constexpr int kStageBytes = GemmCfg<BN, false>::kStageBytes;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
@@ -296,11 +457,12 @@ static bool g_coop_pdl_ok = true;  // cleared if the driver rejects cooperative 
 
 template <int EPI, int BN>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int grid, cudaStream_t stream) {
+    constexpr int kSmem = GemmCfg<BN, gemm_staged<EPI>()>::kSmem;
     static unsigned long long attr_set = 0;  // bit per device
     int dev = 0;
     MMDP_CUDA(cudaGetDevice(&dev));
     if (!(attr_set >> (dev & 63) & 1ull)) {
-        MMDP_CUDA(cudaFuncSetAttribute(gemm_bf16_kernel<EPI, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<BN>::kSmem));
+        MMDP_CUDA(cudaFuncSetAttribute(gemm_bf16_kernel<EPI, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
         attr_set |= 1ull << (dev & 63);
     }
     LaunchScope ls(LK_GEMM, 2.0 * p.M * (double)p.N * p.K, stream);
@@ -308,12 +470,12 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Gem
     // the whole grid or fails the launch; a plain launch could hang behind a concurrent kernel that holds SMs).
     const bool coop = p.sk_tail > 0;
     const bool pdl = pdl_mode() != 0;
-    cudaError_t e = launch_ex(gemm_bf16_kernel<EPI, BN>, dim3(grid), dim3(kGemmThreads), GemmCfg<BN>::kSmem, stream,
+    cudaError_t e = launch_ex(gemm_bf16_kernel<EPI, BN>, dim3(grid), dim3(kGemmThreads), kSmem, stream,
                               pdl && (!coop || g_coop_pdl_ok), coop, tmA, tmB, p);
     if (e != cudaSuccess && coop && pdl && g_coop_pdl_ok) {
         (void)cudaGetLastError();
         g_coop_pdl_ok = false;
-        e = launch_ex(gemm_bf16_kernel<EPI, BN>, dim3(grid), dim3(kGemmThreads), GemmCfg<BN>::kSmem, stream, false, true, tmA, tmB, p);
+        e = launch_ex(gemm_bf16_kernel<EPI, BN>, dim3(grid), dim3(kGemmThreads), kSmem, stream, false, true, tmA, tmB, p);
     }
     if (e != cudaSuccess) return set_error("gemm launch failed: %s", cudaGetErrorString(e));
     MMDP_CUDA(cudaGetLastError());
@@ -399,11 +561,11 @@ static int launch_gemm_pair(const CUtensorMap& tmA, const CUtensorMap& tmBh, con
     MMDP_CUDA(cudaGetDevice(&dev));
     int& mc = max_clusters[dev & 63];
     if (mc == 0) {
-        MMDP_CUDA(cudaFuncSetAttribute(gemm_pair_kernel<EPI, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<BN>::kSmem));
+        MMDP_CUDA(cudaFuncSetAttribute(gemm_pair_kernel<EPI, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<BN, false>::kSmem));
         cudaLaunchConfig_t cfg{};
         cfg.gridDim = dim3(2 * num_sms());
         cfg.blockDim = dim3(kGemmThreads);
-        cfg.dynamicSmemBytes = GemmCfg<BN>::kSmem;
+        cfg.dynamicSmemBytes = GemmCfg<BN, false>::kSmem;
         cudaLaunchAttribute at{};
         at.id = cudaLaunchAttributeClusterDimension;
         at.val.clusterDim.x = 2; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
@@ -414,7 +576,7 @@ static int launch_gemm_pair(const CUtensorMap& tmA, const CUtensorMap& tmBh, con
     }
     const int clusters = pair_tiles < mc ? pair_tiles : mc;
     LaunchScope ls(LK_GEMM, 2.0 * p.M * (double)p.N * p.K, stream);
-    MMDP_CUDA(launch_ex(gemm_pair_kernel<EPI, BN>, dim3(2 * clusters), dim3(kGemmThreads), GemmCfg<BN>::kSmem, stream, pdl_mode() != 0,
+    MMDP_CUDA(launch_ex(gemm_pair_kernel<EPI, BN>, dim3(2 * clusters), dim3(kGemmThreads), GemmCfg<BN, false>::kSmem, stream, pdl_mode() != 0,
                         false, tmA, tmBh, p));
     return 0;
 }

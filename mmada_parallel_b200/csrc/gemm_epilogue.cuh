@@ -1,5 +1,6 @@
-// Fused epilogues of the bf16 GEMM kernel (gemm.cu) and the e4m3 GEMM kernel (fp8.cu). One call handles one thread's wgmma
-// fragment of a 128 x BN accumulator tile held in registers.
+// Fused epilogues of the bf16 GEMM kernel (gemm.cu) and the e4m3 GEMM kernel (fp8.cu). gemm_epilogue_tile handles one thread's
+// wgmma fragment of a 128 x BN accumulator tile held in registers; epi_row8 handles one (row, 8-column) item for the split-K
+// finishing pass and the staged epilogue of gemm_bf16_kernel.
 #pragma once
 #include "mmdp_internal.h"
 #include "ptx.cuh"
@@ -229,122 +230,139 @@ __device__ __forceinline__ void sk_publish(float* __restrict__ slot_ws, const fl
         }
 }
 
+// Row and (sequence, position) of GEMM row `row` for the QKV epilogues (the same mapping as gemm_epilogue_tile's).
+template <int EPI>
+__device__ __forceinline__ void qkv_row_coords(const GemmParams& p, int row, int& b, int& pos) {
+    if constexpr (EPI == EPI_QKVROPE_PACKED) {
+        const int2 sp = p.seg_pos[row];
+        b = sp.x;
+        pos = sp.y;
+    } else if (p.pos_map) {
+        b = row / p.Tq;
+        pos = p.pos_map[row];
+    } else {
+        b = (row + p.row0) / p.L;
+        pos = (row + p.row0) - b * p.L;
+    }
+}
+
+// One work item of the fused epilogue, shared by the split-K finishing pass (fp32 sums) and the staged epilogue of
+// gemm_bf16_kernel (bf16 values from shared memory; every epilogue rounds the accumulator to bf16 first, so both give the
+// same bits as gemm_epilogue_tile): output row `row` (< p.M), 8 consecutive tile columns from `tc`, values v. The rotary and
+// SwiGLU epilogues also take the partner columns w (tc + 64: the other rotary half; tc + 128: the up projection); `rv` is
+// the residual at (row, n_blk * BN + tc) for EPI_RESID, loaded by the caller so that it can batch the loads of its items.
+// Plain / residual / F32 and V items store 8 columns, rotary items 2 x 8, SwiGLU items the 8 products.
+template <int EPI, int BN>
+__device__ __forceinline__ void epi_row8(const GemmParams& p, int row, int n_blk, int tc, const float (&v)[8], const float (&w)[8],
+                                         uint4 rv) {
+    const int n0 = n_blk * BN;
+    if constexpr (EPI == EPI_PLAIN || EPI == EPI_RESID || EPI == EPI_F32) {
+        const int col = n0 + tc;
+        if (col >= p.N) return;
+        if constexpr (EPI == EPI_F32) {
+            float4* d = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.C) + (size_t)row * p.ldc + col);
+            d[0] = make_float4(v[0], v[1], v[2], v[3]);
+            if (col + 4 < p.N) d[1] = make_float4(v[4], v[5], v[6], v[7]);
+        } else {
+            uint32_t o[4];
+            if constexpr (EPI == EPI_RESID) {
+                const uint32_t rr[4] = {rv.x, rv.y, rv.z, rv.w};
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+                    o[i] = pack_bf16x2(__fadd_rn(bf16_lo(rr[i]), bf16_round(v[2 * i])), __fadd_rn(bf16_hi(rr[i]), bf16_round(v[2 * i + 1])));
+            } else {
+#pragma unroll
+                for (int i = 0; i < 4; ++i) o[i] = pack_bf16x2(v[2 * i], v[2 * i + 1]);
+            }
+            *reinterpret_cast<uint4*>(p.C + (size_t)row * p.ldc + col) = make_uint4(o[0], o[1], o[2], o[3]);
+        }
+    } else if constexpr (EPI == EPI_SWIGLU) {
+        const int col = n_blk * (BN / 2) + tc;
+        if (col >= p.N / 2) return;
+        float o[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            const float gg = bf16_round(v[i]), uu = bf16_round(w[i]);
+            const float sl = bf16_round(__fdiv_rn(gg, __fadd_rn(1.0f, expf(-gg))));  // silu -> bf16
+            o[i] = __fmul_rn(sl, uu);
+        }
+        *reinterpret_cast<uint4*>(p.C + (size_t)row * p.ldc + col) =
+            make_uint4(pack_bf16x2(o[0], o[1]), pack_bf16x2(o[2], o[3]), pack_bf16x2(o[4], o[5]), pack_bf16x2(o[6], o[7]));
+    } else if constexpr (EPI == EPI_QKVROPE || EPI == EPI_QKVROPE_PACKED) {
+        const int region = n0 / p.d_model;  // 0 = Q, 1 = K, 2 = V (d_model % 256 == 0 is checked on the host)
+        int b, pos;
+        qkv_row_coords<EPI>(p, row, b, pos);
+        if (region < 2) {
+            const int head = tc >> 7, c = tc & 63;  // tc = head * 128 + c, c < 64
+            const float4* c4 = reinterpret_cast<const float4*>(p.cos_tab + (size_t)pos * 64 + c);
+            const float4* s4 = reinterpret_cast<const float4*>(p.sin_tab + (size_t)pos * 64 + c);
+            const float4 c0 = c4[0], c1 = c4[1], s0 = s4[0], s1 = s4[1];
+            const float cs[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
+            const float sn[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
+            float o1[8], o2[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                const float t1 = bf16_round(v[i]), t2 = bf16_round(w[i]);
+                // (t * cos) + (rotate_half(t) * sin), fp32, no FMA contraction
+                o1[i] = __fadd_rn(__fmul_rn(t1, cs[i]), __fmul_rn(-t2, sn[i]));
+                o2[i] = __fadd_rn(__fmul_rn(t2, cs[i]), __fmul_rn(t1, sn[i]));
+            }
+            const size_t drow = (region == 0 || !p.pos_map) ? (size_t)row : (size_t)b * p.L + pos;  // k rows go to their sequence position
+            __nv_bfloat16* dst = (region == 0 ? p.q : p.k) + drow * p.d_model + (n0 - region * p.d_model) + head * 128 + c;
+            *reinterpret_cast<uint4*>(dst) =
+                make_uint4(pack_bf16x2(o1[0], o1[1]), pack_bf16x2(o1[2], o1[3]), pack_bf16x2(o1[4], o1[5]), pack_bf16x2(o1[6], o1[7]));
+            *reinterpret_cast<uint4*>(dst + 64) =
+                make_uint4(pack_bf16x2(o2[0], o2[1]), pack_bf16x2(o2[2], o2[3]), pack_bf16x2(o2[4], o2[5]), pack_bf16x2(o2[6], o2[7]));
+        } else {
+            // V is written transposed: vt[b][head][d][token] so that P·V runs with both operands K-major
+            const int n = n0 - 2 * p.d_model + tc;
+            const int head = n >> 7, d0 = n & 127;
+            __nv_bfloat16* dst = p.vt + ((size_t)(b * p.n_heads + head) * 128 + d0) * p.Lpad + pos;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) dst[(size_t)i * p.Lpad] = __float2bfloat16_rn(v[i]);
+        }
+    }
+}
+
 template <int EPI, int BN>
 __device__ __forceinline__ void sk_finish(const GemmParams& p, const float4* __restrict__ tile_ws, int S, int unit_s, int m_blk,
                                           int n_blk, int tid) {
     const int r0 = (128 * unit_s) / S, r1 = (128 * (unit_s + 1)) / S;
     const int nrows = r1 - r0;
-    const int n0 = n_blk * BN;
-    if constexpr (EPI == EPI_PLAIN || EPI == EPI_RESID || EPI == EPI_F32) {
-        constexpr int G = BN / 8;
-        for (int idx = tid; idx < nrows * G; idx += kEpiThreads) {
-            const int g = idx / nrows, rit = r0 + idx - g * nrows;
-            const int row = m_blk * 128 + rit, col = n0 + 8 * g;
-            if (row >= p.M || col >= p.N) continue;
-            const int col4[2] = {2 * g, 2 * g + 1};
-            float4 a[2];
-            sk_sum<BN, 2>(tile_ws, S, rit, col4, a);
-            if constexpr (EPI == EPI_F32) {
-                float4* d = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.C) + (size_t)row * p.ldc + col);
-                d[0] = a[0];
-                if (col + 4 < p.N) d[1] = a[1];
-            } else {
-                const float f[8] = {a[0].x, a[0].y, a[0].z, a[0].w, a[1].x, a[1].y, a[1].z, a[1].w};
-                uint32_t o[4];
-                if constexpr (EPI == EPI_RESID) {
-                    const uint4 rv = *reinterpret_cast<const uint4*>(p.resid + (size_t)row * p.ldr + col);
-                    const uint32_t rr[4] = {rv.x, rv.y, rv.z, rv.w};
-#pragma unroll
-                    for (int i = 0; i < 4; ++i)
-                        o[i] = pack_bf16x2(__fadd_rn(bf16_lo(rr[i]), bf16_round(f[2 * i])), __fadd_rn(bf16_hi(rr[i]), bf16_round(f[2 * i + 1])));
-                } else {
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) o[i] = pack_bf16x2(f[2 * i], f[2 * i + 1]);
-                }
-                *reinterpret_cast<uint4*>(p.C + (size_t)row * p.ldc + col) = make_uint4(o[0], o[1], o[2], o[3]);
-            }
-        }
-    } else if constexpr (EPI == EPI_SWIGLU) {
-        constexpr int G = 16;  // 128 output columns per tile
-        for (int idx = tid; idx < nrows * G; idx += kEpiThreads) {
-            const int g = idx / nrows, rit = r0 + idx - g * nrows;
-            const int row = m_blk * 128 + rit, col = n_blk * 128 + 8 * g;
-            if (row >= p.M || col >= p.N / 2) continue;
-            const int col4[4] = {2 * g, 2 * g + 1, 32 + 2 * g, 32 + 2 * g + 1};
+    // items per tile row: 8-column groups; the rotary (q / k) and SwiGLU items carry their partner columns
+    const bool pair = EPI == EPI_SWIGLU || ((EPI == EPI_QKVROPE || EPI == EPI_QKVROPE_PACKED) && n_blk * BN < 2 * p.d_model);
+    const int G = pair ? 16 : BN / 8;
+    for (int idx = tid; idx < nrows * G; idx += kEpiThreads) {
+        const int g = idx / nrows, rit = r0 + idx - g * nrows;
+        const int row = m_blk * 128 + rit;
+        if (row >= p.M) continue;
+        // tile column of the item and of its partner: SwiGLU g -> 8g, +128; rotary g = (head, gg) -> 128 head + 8 gg, +64
+        const int tc = EPI == EPI_SWIGLU ? 8 * g : (pair ? (g >> 3) * 128 + 8 * (g & 7) : 8 * g);
+        const int tw = EPI == EPI_SWIGLU ? tc + 128 : tc + 64;
+        float v[8], w[8];
+        if (pair) {
+            const int col4[4] = {tc / 4, tc / 4 + 1, tw / 4, tw / 4 + 1};
             float4 a[4];
             sk_sum<BN, 4>(tile_ws, S, rit, col4, a);
-            const float gt[8] = {a[0].x, a[0].y, a[0].z, a[0].w, a[1].x, a[1].y, a[1].z, a[1].w};
-            const float up[8] = {a[2].x, a[2].y, a[2].z, a[2].w, a[3].x, a[3].y, a[3].z, a[3].w};
-            float o[8];
+            const float4 av[4] = {a[0], a[1], a[2], a[3]};
 #pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const float gg = bf16_round(gt[i]), uu = bf16_round(up[i]);
-                const float sl = bf16_round(__fdiv_rn(gg, __fadd_rn(1.0f, expf(-gg))));  // silu -> bf16
-                o[i] = __fmul_rn(sl, uu);
-            }
-            *reinterpret_cast<uint4*>(p.C + (size_t)row * p.ldc + col) =
-                make_uint4(pack_bf16x2(o[0], o[1]), pack_bf16x2(o[2], o[3]), pack_bf16x2(o[4], o[5]), pack_bf16x2(o[6], o[7]));
-        }
-    } else if constexpr (EPI == EPI_QKVROPE || EPI == EPI_QKVROPE_PACKED) {
-        const int region = n0 / p.d_model;  // 0 = Q, 1 = K, 2 = V
-        if (region < 2) {
-            constexpr int G = 16;  // 2 heads x 8 column groups of the first half
-            __nv_bfloat16* base = (region == 0 ? p.q : p.k) + (n0 - region * p.d_model);
-            for (int idx = tid; idx < nrows * G; idx += kEpiThreads) {
-                const int g = idx / nrows, rit = r0 + idx - g * nrows;
-                const int row = m_blk * 128 + rit;
-                if (row >= p.M) continue;
-                const int head = g >> 3, gg = g & 7;
-                const int col4[4] = {head * 32 + 2 * gg, head * 32 + 2 * gg + 1, head * 32 + 16 + 2 * gg, head * 32 + 16 + 2 * gg + 1};
-                float4 a[4];
-                sk_sum<BN, 4>(tile_ws, S, rit, col4, a);
-                const int pos = EPI == EPI_QKVROPE_PACKED ? p.seg_pos[row].y : (row + p.row0) % p.L;
-                const float4* c4 = reinterpret_cast<const float4*>(p.cos_tab + (size_t)pos * 64 + 8 * gg);
-                const float4* s4 = reinterpret_cast<const float4*>(p.sin_tab + (size_t)pos * 64 + 8 * gg);
-                const float4 c0 = c4[0], c1 = c4[1], s0 = s4[0], s1 = s4[1];
-                const float cs[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
-                const float sn[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-                const float x1[8] = {a[0].x, a[0].y, a[0].z, a[0].w, a[1].x, a[1].y, a[1].z, a[1].w};
-                const float x2[8] = {a[2].x, a[2].y, a[2].z, a[2].w, a[3].x, a[3].y, a[3].z, a[3].w};
-                float o1[8], o2[8];
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const float t1 = bf16_round(x1[i]), t2 = bf16_round(x2[i]);
-                    o1[i] = __fadd_rn(__fmul_rn(t1, cs[i]), __fmul_rn(-t2, sn[i]));
-                    o2[i] = __fadd_rn(__fmul_rn(t2, cs[i]), __fmul_rn(t1, sn[i]));
-                }
-                __nv_bfloat16* dst = base + (size_t)row * p.d_model + head * 128 + 8 * gg;
-                *reinterpret_cast<uint4*>(dst) =
-                    make_uint4(pack_bf16x2(o1[0], o1[1]), pack_bf16x2(o1[2], o1[3]), pack_bf16x2(o1[4], o1[5]), pack_bf16x2(o1[6], o1[7]));
-                *reinterpret_cast<uint4*>(dst + 64) =
-                    make_uint4(pack_bf16x2(o2[0], o2[1]), pack_bf16x2(o2[2], o2[3]), pack_bf16x2(o2[4], o2[5]), pack_bf16x2(o2[6], o2[7]));
+            for (int i = 0; i < 2; ++i) {
+                v[4 * i] = av[i].x; v[4 * i + 1] = av[i].y; v[4 * i + 2] = av[i].z; v[4 * i + 3] = av[i].w;
+                w[4 * i] = av[2 + i].x; w[4 * i + 1] = av[2 + i].y; w[4 * i + 2] = av[2 + i].z; w[4 * i + 3] = av[2 + i].w;
             }
         } else {
-            constexpr int G = BN / 8;
-            for (int idx = tid; idx < nrows * G; idx += kEpiThreads) {
-                const int g = idx / nrows, rit = r0 + idx - g * nrows;
-                const int row = m_blk * 128 + rit;
-                if (row >= p.M) continue;
-                const int col4[2] = {2 * g, 2 * g + 1};
-                float4 a[2];
-                sk_sum<BN, 2>(tile_ws, S, rit, col4, a);
-                int b, pos;
-                if constexpr (EPI == EPI_QKVROPE_PACKED) {
-                    const int2 sp = p.seg_pos[row];
-                    b = sp.x;
-                    pos = sp.y;
-                } else {
-                    b = (row + p.row0) / p.L;
-                    pos = (row + p.row0) - b * p.L;
-                }
-                const int n = n0 - 2 * p.d_model + 8 * g;
-                const int head = n >> 7, d0 = n & 127;
-                __nv_bfloat16* dst = p.vt + ((size_t)(b * p.n_heads + head) * 128 + d0) * p.Lpad + pos;
-                const float f[8] = {a[0].x, a[0].y, a[0].z, a[0].w, a[1].x, a[1].y, a[1].z, a[1].w};
+            if (n_blk * BN + tc >= p.N) continue;
+            const int col4[2] = {tc / 4, tc / 4 + 1};
+            float4 a[2];
+            sk_sum<BN, 2>(tile_ws, S, rit, col4, a);
 #pragma unroll
-                for (int i = 0; i < 8; ++i) dst[(size_t)i * p.Lpad] = __float2bfloat16_rn(f[i]);
-            }
+            for (int i = 0; i < 2; ++i) { v[4 * i] = a[i].x; v[4 * i + 1] = a[i].y; v[4 * i + 2] = a[i].z; v[4 * i + 3] = a[i].w; }
+#pragma unroll
+            for (int i = 0; i < 8; ++i) w[i] = 0.f;
         }
+        uint4 rv = make_uint4(0, 0, 0, 0);
+        if constexpr (EPI == EPI_RESID) rv = *reinterpret_cast<const uint4*>(p.resid + (size_t)row * p.ldr + n_blk * BN + tc);
+        epi_row8<EPI, BN>(p, row, n_blk, tc, v, w, rv);
     }
 }
 
