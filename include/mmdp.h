@@ -173,6 +173,14 @@ MMDP_API int mmdp_qkv_rope(const uint16_t* A, int lda, const uint16_t* Wqkv, int
 MMDP_API int mmdp_qkv_rope_tp(const uint16_t* A, int lda, const uint16_t* Wqkv, int M, int d_model, int n_heads_local, int L,
                       int Lpad, const float* cos_tab, const float* sin_tab, uint16_t* q, uint16_t* k, uint16_t* vt, void* stream);
 
+/* Grouped-query form of mmdp_qkv_rope (modeling_llada.py:872-884): n_kv_heads divides n_heads, d_kv = 128 * n_kv_heads.
+ * Wqkv = [q_proj; k_proj; v_proj] rows ([d_model + 2*d_kv, d_model]); bias (nullable) = [q_bias; k_bias; v_bias] bf16
+ * [d_model + 2*d_kv], added to the fp32 accumulator before the bf16 rounding (nn.Linear with bias). Outputs q [B*L, d_model],
+ * k [B*L, d_kv] (RoPE applied), vt [B, n_kv_heads, 128, Lpad]. */
+MMDP_API int mmdp_qkv_rope_gqa(const uint16_t* A, int lda, const uint16_t* Wqkv, const uint16_t* bias, int M, int d_model, int n_heads,
+                               int n_kv_heads, int L, int Lpad, const float* cos_tab, const float* sin_tab, uint16_t* q, uint16_t* k,
+                               uint16_t* vt, void* stream);
+
 /* x = bf16(bf16(partial) + x): residual add of an fp32 partial-sum buffer that was all-reduced across tensor-parallel ranks
  * (keeps the reference's rounding points: nn.Linear output -> bf16, then the residual add -> bf16). */
 MMDP_API int mmdp_resid_add_f32(uint16_t* x, int ldx, const float* partial, int ldp, int M, int d, void* stream);
@@ -188,6 +196,12 @@ MMDP_API int mmdp_attention(const uint16_t* q, const uint16_t* k, const uint16_t
  * attends to its own keys only; its pad columns vt[i, ..., seg_len[i]:Lpad] must hold finite values (they meet P == 0). */
 MMDP_API int mmdp_attention_packed(const uint16_t* q, const uint16_t* k, const uint16_t* vt, uint16_t* out, int n_seg, const int32_t* seg_len,
                                    int n_heads, int Lpad, float scale, void* stream);
+/* Grouped-query attention (modeling_llada.py:660-679: k / v repeat_interleave'd to n_heads): n_kv_heads divides n_heads and query
+ * head h attends with kv head h / (n_heads / n_kv_heads). k: [rows, n_kv_heads*128]; vt: [B or n_seg, n_kv_heads, 128, Lpad];
+ * q / out as above. seg_len == NULL: B sequences of L rows each (mmdp_attention); otherwise the packed batch of n_seg = B
+ * sequences (mmdp_attention_packed, L ignored). n_kv_heads == n_heads runs the multi-head kernels. */
+MMDP_API int mmdp_attention_gqa(const uint16_t* q, const uint16_t* k, const uint16_t* vt, uint16_t* out, int B, const int32_t* seg_len,
+                                int n_heads, int n_kv_heads, int L, int Lpad, float scale, void* stream);
 
 /* RMSLayerNorm.forward (modeling_llada.py:315-329). rows (nullable int32[M]) gathers input rows. */
 MMDP_API int mmdp_rmsnorm(const uint16_t* x, int ldx, const int32_t* rows, const uint16_t* weight, uint16_t* y, int ldy, int M,
@@ -349,13 +363,22 @@ MMDP_API int mmdp_model_create(const mmdp_model_config* cfg, mmdp_model** out);
 #define MMDP_PRECISION_BF16 0
 #define MMDP_PRECISION_FP8 1
 MMDP_API int mmdp_model_create_ex(const mmdp_model_config* cfg, int precision, mmdp_model** out);
+/* Attention layout of the blocks (mmdp_model_create / _ex mean n_kv_heads = n_heads, flags = 0):
+ *   n_kv_heads   kv heads (effective_n_kv_heads of the reference config; divides n_heads): k_proj / v_proj are
+ *                [d_kv, d] with d_kv = 128 * n_kv_heads and query head h attends with kv head h / (n_heads / n_kv_heads);
+ *   flags        MMDP_ARCH_QKV_BIAS: q_proj / k_proj / v_proj carry a bias (config.include_qkv_bias), loaded as
+ *                "blocks.<i>.q_bias|k_bias|v_bias" ([d], [d_kv], [d_kv]).
+ * Such a context runs mmdp_model_forward, _window and _packed in both precisions; mmdp_model_forward_cached is refused. */
+#define MMDP_ARCH_QKV_BIAS 1
+MMDP_API int mmdp_model_create_arch(const mmdp_model_config* cfg, int precision, int n_kv_heads, int flags, mmdp_model** out);
 MMDP_API void mmdp_model_destroy(mmdp_model* m);
 
 /* Copies (and packs) one tensor of the HF state dict into the model-owned device buffers. `src` may be a device or
  * a pinned/pageable host pointer (cudaMemcpyDefault). Names (layer = 0..n_layers-1):
  *   "wte" [V,d], "ln_f" [d], "head" [V,d],
  *   "blocks.<i>.q_proj|k_proj|v_proj|attn_out" [d,d], "blocks.<i>.ff_proj|up_proj" [ff,d], "blocks.<i>.ff_out" [d,ff],
- *   "blocks.<i>.attn_norm|ff_norm" [d]. */
+ *   "blocks.<i>.attn_norm|ff_norm" [d]; in a grouped-query context k_proj / v_proj are [d_kv, d], and with
+ *   MMDP_ARCH_QKV_BIAS "blocks.<i>.q_bias" [d] and "blocks.<i>.k_bias|v_bias" [d_kv] are expected too. */
 MMDP_API int mmdp_model_set_weight(mmdp_model* m, const char* name, const void* src, int64_t rows, int64_t cols, void* stream);
 
 /* fp32 rotary tables [L, 64] (cos, sin), computed by the host exactly like RotaryEmbedding.get_rotary_embedding. */

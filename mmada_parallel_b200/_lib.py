@@ -17,6 +17,7 @@ LIB_PATH = os.path.join(_HERE, "libmmdp.so")
 
 EPI_PLAIN, EPI_RESID, EPI_SWIGLU, EPI_F32 = 0, 1, 3, 4
 PRECISION_BF16, PRECISION_FP8 = 0, 1
+ARCH_QKV_BIAS = 1  # mmdp_model_create_arch flags
 
 
 class MmdpError(RuntimeError):
@@ -103,9 +104,11 @@ SIGNATURES = {
     "mmdp_gemm_fp8": (_i, [_i, _vp, _i, _vp, _vp, _i, _vp, _i, _i, _i, _vp, _i, _vp, _i, _vp]),
     "mmdp_qkv_rope": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mmdp_qkv_rope_tp": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "mmdp_qkv_rope_gqa": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mmdp_resid_add_f32": (_i, [_vp, _i, _vp, _i, _i, _i, _vp]),
     "mmdp_attention": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp]),
     "mmdp_attention_packed": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _f, _vp]),
+    "mmdp_attention_gqa": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _f, _vp]),
     "mmdp_rmsnorm": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _f, _vp]),
     "mmdp_embed": (_i, [_vp, _vp, _vp, _i, _i, _i64, _vp]),
     "mmdp_text_step": (_i, [_vp, _vp, _i64, _i, _i, _f, _vp, _i64, _f, _vp, _i64, _i, _vp, _vp, _vp]),
@@ -131,6 +134,7 @@ SIGNATURES = {
     "mmdp_vq_nearest": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "mmdp_model_create": (_i, [C.POINTER(ModelConfig), C.POINTER(_vp)]),
     "mmdp_model_create_ex": (_i, [C.POINTER(ModelConfig), _i, C.POINTER(_vp)]),
+    "mmdp_model_create_arch": (_i, [C.POINTER(ModelConfig), _i, _i, _i, C.POINTER(_vp)]),
     "mmdp_model_destroy": (None, [_vp]),
     "mmdp_model_set_weight": (_i, [_vp, C.c_char_p, _vp, _i64, _i64, _vp]),
     "mmdp_model_set_rope": (_i, [_vp, _vp, _vp, _i, _vp]),
@@ -256,6 +260,35 @@ def attention_packed(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, seq_len
     out = torch.empty_like(q)
     check(lib.mmdp_attention_packed(ptr(q), ptr(k), ptr(vt), ptr(out), len(seq_lens), lens, n_heads, vt.shape[-1], scale,
                                     stream_ptr()))
+    return out
+
+
+def qkv_rope_gqa(a: torch.Tensor, wqkv: torch.Tensor, bias: Optional[torch.Tensor], n_heads: int, n_kv_heads: int, L: int,
+                 cos: torch.Tensor, sin: torch.Tensor):
+    """Grouped-query q/k/v projection + RoPE: wqkv [d + 2 d_kv, d], bias (optional) [d + 2 d_kv] -> q [M, d], k [M, d_kv],
+    vt [B, n_kv_heads, 128, Lpad] (pad columns zero)."""
+    require_cuda(a, wqkv, bias, cos, sin)
+    M, d = a.shape
+    B = M // L
+    Lpad = (L + 7) // 8 * 8
+    q = torch.empty((M, d), dtype=torch.bfloat16, device=a.device)
+    k = torch.empty((M, 128 * n_kv_heads), dtype=torch.bfloat16, device=a.device)
+    vt = torch.zeros((B, n_kv_heads, 128, Lpad), dtype=torch.bfloat16, device=a.device)
+    check(lib.mmdp_qkv_rope_gqa(ptr(a), a.stride(0), ptr(wqkv), ptr(bias), M, d, n_heads, n_kv_heads, L, Lpad, ptr(cos), ptr(sin),
+                                ptr(q), ptr(k), ptr(vt), stream_ptr()))
+    return q, k, vt
+
+
+def attention_gqa(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, n_heads: int, n_kv_heads: int, scale: float, B: int = 1,
+                  L: int = 0, seq_lens=None) -> torch.Tensor:
+    """Grouped-query attention: q [rows, n_heads * 128], k [rows, n_kv_heads * 128], vt [B or len(seq_lens), n_kv_heads, 128, Lpad].
+    seq_lens None: B sequences of L rows; otherwise a packed batch."""
+    require_cuda(q, k, vt)
+    out = torch.empty_like(q)
+    lens = None if seq_lens is None else (C.c_int32 * len(seq_lens))(*[int(x) for x in seq_lens])
+    nb = B if seq_lens is None else len(seq_lens)
+    check(lib.mmdp_attention_gqa(ptr(q), ptr(k), ptr(vt), ptr(out), nb, lens, n_heads, n_kv_heads, L, vt.shape[-1], scale,
+                                 stream_ptr()))
     return out
 
 

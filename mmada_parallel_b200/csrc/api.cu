@@ -54,7 +54,7 @@ int lfq_decode(const int64_t* ids, float* zq, int B, int N, int bits, cudaStream
 }  // namespace mmdp
 
 struct LayerWeights {
-    bf16* wqkv;       // [3d, d]   rows: q_proj | k_proj | v_proj
+    bf16* wqkv;       // [d + 2 d_kv, d]   rows: q_proj | k_proj | v_proj (d_kv = 128 n_kv_heads; d in a multi-head context)
     bf16* wo;         // [d, d]
     bf16* w13;        // [2ff, d]  128-row blocks interleaved: ff_proj block t, up_proj block t
     bf16* w2;         // [d, ff]
@@ -64,10 +64,16 @@ struct LayerWeights {
     // of the FP8 GEMM's 128-wide tile) with one fp32 scale per row; the bf16 pointers above are then null
     uint8_t *wqkv8 = nullptr, *wo8 = nullptr, *w13_8 = nullptr, *w2_8 = nullptr;
     float *sqkv = nullptr, *so = nullptr, *s13 = nullptr, *s2 = nullptr;
+    bf16* qkv_bias = nullptr;  // MMDP_ARCH_QKV_BIAS: [d + 2 d_kv], q_bias | k_bias | v_bias
 };
 
 struct mmdp_model {
     mmdp_model_config cfg;
+    // attention layout (mmdp_model_create_arch): kv heads and MMDP_ARCH_* flags. A context with n_kv_heads < n_heads or a bias
+    // runs the grouped-query QKV epilogues; a plain multi-head one keeps EPI_QKVROPE(_PACKED)
+    int n_kv_heads = 0, flags = 0;
+    int d_kv() const { return n_kv_heads * 128; }
+    bool gqa() const { return n_kv_heads != cfg.n_heads || flags != 0; }
     std::vector<LayerWeights> layers;
     bf16* wte = nullptr;
     bf16* ln_f = nullptr;
@@ -128,6 +134,16 @@ MMDP_API int mmdp_qkv_rope(const uint16_t* A, int lda, const uint16_t* Wqkv, int
                      nullptr, 0, &qa, (cudaStream_t)stream);
 }
 
+MMDP_API int mmdp_qkv_rope_gqa(const uint16_t* A, int lda, const uint16_t* Wqkv, const uint16_t* bias, int M, int d_model, int n_heads,
+                               int n_kv_heads, int L, int Lpad, const float* cos_tab, const float* sin_tab, uint16_t* q, uint16_t* k,
+                               uint16_t* vt, void* stream) {
+    QkvRopeArgs qa{(bf16*)q, (bf16*)k, (bf16*)vt, cos_tab, sin_tab, L, Lpad, d_model, n_heads};
+    qa.n_kv_heads = n_kv_heads;
+    qa.bias = (const bf16*)bias;
+    return gemm_bf16(EPI_QKVGQA, (const bf16*)A, lda, (const bf16*)Wqkv, d_model, M, d_model + 2 * 128 * n_kv_heads, d_model, nullptr, 0,
+                     nullptr, 0, &qa, (cudaStream_t)stream);
+}
+
 MMDP_API int mmdp_qkv_rope_tp(const uint16_t* A, int lda, const uint16_t* Wqkv, int M, int d_model, int n_heads_local, int L,
                       int Lpad, const float* cos_tab, const float* sin_tab, uint16_t* q, uint16_t* k, uint16_t* vt, void* stream) {
     const int d_attn = n_heads_local * 128;
@@ -153,6 +169,20 @@ MMDP_API int mmdp_attention_packed(const uint16_t* q, const uint16_t* k, const u
     segs.n = n_seg;
     for (int i = 0; i < n_seg; ++i) segs.start[i + 1] = segs.start[i] + seg_len[i];
     return attention_packed_fwd((const bf16*)q, (const bf16*)k, (const bf16*)vt, (bf16*)out, segs, n_heads, Lpad, scale, (cudaStream_t)stream);
+}
+
+MMDP_API int mmdp_attention_gqa(const uint16_t* q, const uint16_t* k, const uint16_t* vt, uint16_t* out, int B, const int32_t* seg_len,
+                                int n_heads, int n_kv_heads, int L, int Lpad, float scale, void* stream) {
+    if (n_kv_heads <= 0) return set_error("mmdp_attention_gqa: n_kv_heads must be positive");
+    if (!seg_len)
+        return attention_fwd((const bf16*)q, (const bf16*)k, (const bf16*)vt, (bf16*)out, B, n_heads, L, Lpad, scale, (cudaStream_t)stream, 0,
+                             n_kv_heads);
+    if (B <= 0 || B > kMaxSegs) return set_error("mmdp_attention_gqa: %d sequences (1 to %d)", B, kMaxSegs);
+    SegTable segs{};
+    segs.n = B;
+    for (int i = 0; i < B; ++i) segs.start[i + 1] = segs.start[i] + seg_len[i];
+    return attention_packed_fwd((const bf16*)q, (const bf16*)k, (const bf16*)vt, (bf16*)out, segs, n_heads, Lpad, scale, (cudaStream_t)stream,
+                                n_kv_heads);
 }
 
 MMDP_API int mmdp_rmsnorm(const uint16_t* x, int ldx, const int32_t* rows, const uint16_t* weight, uint16_t* y, int ldy, int M,
@@ -379,7 +409,15 @@ MMDP_API int mmdp_model_create(const mmdp_model_config* c, mmdp_model** out) {
 }
 
 MMDP_API int mmdp_model_create_ex(const mmdp_model_config* c, int precision, mmdp_model** out) {
+    if (!c) return set_error("mmdp_model_create: null argument");
+    return mmdp_model_create_arch(c, precision, c->n_heads, 0, out);
+}
+
+MMDP_API int mmdp_model_create_arch(const mmdp_model_config* c, int precision, int n_kv_heads, int flags, mmdp_model** out) {
     if (!c || !out) return set_error("mmdp_model_create: null argument");
+    if (n_kv_heads <= 0 || n_kv_heads > c->n_heads || c->n_heads % n_kv_heads)
+        return set_error("mmdp_model_create: n_kv_heads=%d must divide n_heads=%d", n_kv_heads, c->n_heads);
+    if (flags & ~MMDP_ARCH_QKV_BIAS) return set_error("mmdp_model_create: unknown architecture flags 0x%x", flags);
     if (precision != MMDP_PRECISION_BF16 && precision != MMDP_PRECISION_FP8)
         return set_error("mmdp_model_create: unknown precision %d", precision);
     if (c->d_model != c->n_heads * 128) return set_error("mmdp_model_create: head_dim must be 128");
@@ -394,21 +432,24 @@ MMDP_API int mmdp_model_create_ex(const mmdp_model_config* c, int precision, mmd
     mmdp_model* m = new mmdp_model();
     m->cfg = *c;
     m->precision = precision;
-    const size_t d = c->d_model, ff = c->mlp_hidden, V = c->vocab_size;
+    m->n_kv_heads = n_kv_heads;
+    m->flags = flags;
+    const size_t d = c->d_model, ff = c->mlp_hidden, V = c->vocab_size, dkv = m->d_kv(), nqkv = d + 2 * dkv;
     m->layers.resize(c->n_layers);
     int rc = 0;
     for (auto& l : m->layers) {
+        if (flags & MMDP_ARCH_QKV_BIAS) rc |= dev_alloc(m, (void**)&l.qkv_bias, nqkv * 2);
         if (precision == MMDP_PRECISION_FP8) {
-            rc |= dev_alloc(m, (void**)&l.wqkv8, 3 * d * d);
+            rc |= dev_alloc(m, (void**)&l.wqkv8, nqkv * d);
             rc |= dev_alloc(m, (void**)&l.wo8, d * d);
             rc |= dev_alloc(m, (void**)&l.w13_8, 2 * ff * d);
             rc |= dev_alloc(m, (void**)&l.w2_8, d * ff);
-            rc |= dev_alloc(m, (void**)&l.sqkv, 3 * d * 4);
+            rc |= dev_alloc(m, (void**)&l.sqkv, nqkv * 4);
             rc |= dev_alloc(m, (void**)&l.so, d * 4);
             rc |= dev_alloc(m, (void**)&l.s13, 2 * ff * 4);
             rc |= dev_alloc(m, (void**)&l.s2, d * 4);
         } else {
-            rc |= dev_alloc(m, (void**)&l.wqkv, 3 * d * d * 2);
+            rc |= dev_alloc(m, (void**)&l.wqkv, nqkv * d * 2);
             rc |= dev_alloc(m, (void**)&l.wo, d * d * 2);
             rc |= dev_alloc(m, (void**)&l.w13, 2 * ff * d * 2);
             rc |= dev_alloc(m, (void**)&l.w2, d * ff * 2);
@@ -425,7 +466,7 @@ MMDP_API int mmdp_model_create_ex(const mmdp_model_config* c, int precision, mmd
     rc |= dev_alloc(m, (void**)&m->x, Mm * d * 2);
     rc |= dev_alloc(m, (void**)&m->xn, Mm * d * 2);
     rc |= dev_alloc(m, (void**)&m->q, Mm * d * 2);
-    rc |= dev_alloc(m, (void**)&m->k, Mm * d * 2);
+    rc |= dev_alloc(m, (void**)&m->k, Mm * dkv * 2);
     rc |= dev_alloc(m, (void**)&m->att, Mm * d * 2);
     rc |= dev_alloc(m, (void**)&m->xr, Mm * d * 2);
     rc |= dev_alloc(m, (void**)&m->h, Mm * ff * 2);
@@ -433,7 +474,7 @@ MMDP_API int mmdp_model_create_ex(const mmdp_model_config* c, int precision, mmd
         rc |= dev_alloc(m, (void**)&m->a8, Mm * ff);
         rc |= dev_alloc(m, (void**)&m->as, Mm * (ff / 128) * 4);
     }
-    rc |= dev_alloc(m, (void**)&m->vt, (size_t)c->max_batch * d * m->Lpad_max * 2);
+    rc |= dev_alloc(m, (void**)&m->vt, (size_t)c->max_batch * dkv * m->Lpad_max * 2);
     rc |= dev_alloc(m, (void**)&m->cos_tab, (size_t)c->max_seq_len * 64 * 4);
     rc |= dev_alloc(m, (void**)&m->sin_tab, (size_t)c->max_seq_len * 64 * 4);
     rc |= dev_alloc(m, (void**)&m->err_flag, sizeof(int));
@@ -461,7 +502,8 @@ static int copy_rows(void* dst, const void* src, size_t bytes, cudaStream_t s) {
 
 // FP8 context: one linear of a block [rows, cols] (bf16, device or host) -> e4m3 with one scale per row (group = cols), written
 // into the packed layer matrices. The bf16 source is staged on the device and never kept.
-static int set_weight_fp8(LayerWeights& l, const char* sub, const void* src, int64_t rows, int64_t cols, cudaStream_t s) {
+// qkv_row0: first row of q_proj / k_proj / v_proj inside the packed Wqkv (0, d, d + d_kv)
+static int set_weight_fp8(LayerWeights& l, const char* sub, const void* src, int64_t rows, int64_t cols, int64_t qkv_row0, cudaStream_t s) {
     const size_t n = (size_t)rows * cols;
     const bool w13 = !strcmp(sub, "up_proj") || !strcmp(sub, "ff_proj");
     bf16* stage = nullptr;
@@ -472,9 +514,8 @@ static int set_weight_fp8(LayerWeights& l, const char* sub, const void* src, int
     if (!strcmp(sub, "attn_out")) { q = l.wo8; sc = l.so; }
     else if (!strcmp(sub, "ff_out")) { q = l.w2_8; sc = l.s2; }
     else if (!w13) {
-        const int which = sub[0] == 'q' ? 0 : (sub[0] == 'k' ? 1 : 2);
-        q = l.wqkv8 + (size_t)which * n;
-        sc = l.sqkv + (size_t)which * rows;
+        q = l.wqkv8 + (size_t)qkv_row0 * cols;
+        sc = l.sqkv + qkv_row0;
     } else {  // quantised next to the stage, then interleaved: source block t of 64 rows -> destination block 2t + up
         q = reinterpret_cast<uint8_t*>(stage + n);
         sc = reinterpret_cast<float*>(q + n);
@@ -495,7 +536,7 @@ static int set_weight_fp8(LayerWeights& l, const char* sub, const void* src, int
 MMDP_API int mmdp_model_set_weight(mmdp_model* m, const char* name, const void* src, int64_t rows, int64_t cols, void* stream) {
     if (!m || !name || !src) return set_error("mmdp_model_set_weight: null argument");
     cudaStream_t s = (cudaStream_t)stream;
-    const int64_t d = m->cfg.d_model, ff = m->cfg.mlp_hidden, V = m->cfg.vocab_size;
+    const int64_t d = m->cfg.d_model, ff = m->cfg.mlp_hidden, V = m->cfg.vocab_size, dkv = m->d_kv();
     auto expect = [&](int64_t r, int64_t c) -> int {
         if (rows != r || cols != c)
             return set_error("mmdp_model_set_weight(%s): expected [%lld,%lld], got [%lld,%lld]", name, (long long)r,
@@ -511,20 +552,26 @@ MMDP_API int mmdp_model_set_weight(mmdp_model* m, const char* name, const void* 
     if (sscanf(name, "blocks.%d.%63s", &li, sub) != 2 || li < 0 || li >= m->cfg.n_layers)
         return set_error("mmdp_model_set_weight: unknown tensor name '%s'", name);
     LayerWeights& l = m->layers[li];
+    // q_proj | k_proj | v_proj rows of the packed Wqkv (and of the bias): [0, d), [d, d + d_kv), [d + d_kv, d + 2 d_kv)
+    const bool qkv = !strcmp(sub, "q_proj") || !strcmp(sub, "k_proj") || !strcmp(sub, "v_proj");
+    const int64_t qkv_row0 = sub[0] == 'q' ? 0 : (sub[0] == 'k' ? d : d + dkv), qkv_rows = sub[0] == 'q' ? d : dkv;
+    if (!strcmp(sub, "q_bias") || !strcmp(sub, "k_bias") || !strcmp(sub, "v_bias")) {
+        if (!l.qkv_bias) return set_error("mmdp_model_set_weight(%s): the context was created without MMDP_ARCH_QKV_BIAS", name);
+        if (expect(qkv_rows, 1) && expect(1, qkv_rows)) return -1;
+        return copy_rows(l.qkv_bias + qkv_row0, src, qkv_rows * 2, s);
+    }
     if (m->precision == MMDP_PRECISION_FP8) {
-        const bool qkv = !strcmp(sub, "q_proj") || !strcmp(sub, "k_proj") || !strcmp(sub, "v_proj");
         const bool w13 = !strcmp(sub, "ff_proj") || !strcmp(sub, "up_proj");
         const bool wo = !strcmp(sub, "attn_out"), w2 = !strcmp(sub, "ff_out");
         if (qkv || w13 || wo || w2) {
-            const int64_t r = w13 ? ff : d, k = w2 ? ff : d;
+            const int64_t r = w13 ? ff : (qkv ? qkv_rows : d), k = w2 ? ff : d;
             if (expect(r, k)) return -1;
-            return set_weight_fp8(l, sub, src, r, k, s);
+            return set_weight_fp8(l, sub, src, r, k, qkv_row0, s);
         }
     }
-    if (!strcmp(sub, "q_proj") || !strcmp(sub, "k_proj") || !strcmp(sub, "v_proj")) {
-        if (expect(d, d)) return -1;
-        const int which = sub[0] == 'q' ? 0 : (sub[0] == 'k' ? 1 : 2);
-        return copy_rows(l.wqkv + (size_t)which * d * d, src, d * d * 2, s);
+    if (qkv) {
+        if (expect(qkv_rows, d)) return -1;
+        return copy_rows(l.wqkv + (size_t)qkv_row0 * d, src, qkv_rows * d * 2, s);
     }
     if (!strcmp(sub, "attn_out")) { if (expect(d, d)) return -1; return copy_rows(l.wo, src, d * d * 2, s); }
     if (!strcmp(sub, "ff_out")) { if (expect(d, ff)) return -1; return copy_rows(l.w2, src, d * ff * 2, s); }
@@ -570,7 +617,7 @@ enum { LIN_QKV = 0, LIN_O = 1, LIN_13 = 2, LIN_2 = 3 };
 static int block_linear(mmdp_model* m, const LayerWeights& l, int which, int epi, const bf16* A, int lda, int M, bf16* C, int ldc,
                         const bf16* R, int ldr, const QkvRopeArgs* qa, cudaStream_t s) {
     const int d = m->cfg.d_model, ff = m->cfg.mlp_hidden;
-    const int N = which == LIN_QKV ? 3 * d : (which == LIN_13 ? 2 * ff : d);
+    const int N = which == LIN_QKV ? d + 2 * m->d_kv() : (which == LIN_13 ? 2 * ff : d);
     const int K = which == LIN_2 ? ff : d;
     if (m->precision == MMDP_PRECISION_BF16) {
         const bf16* W = which == LIN_QKV ? l.wqkv : (which == LIN_O ? l.wo : (which == LIN_13 ? l.w13 : l.w2));
@@ -582,7 +629,7 @@ static int block_linear(mmdp_model* m, const LayerWeights& l, int which, int epi
     return gemm_fp8(epi, m->a8, K, m->as, W, K, sw, M, N, K, C, ldc, R, ldr, qa, s);
 }
 
-// V^T pad rule. Block s of m->vt ([max_batch][H][128][Lpad], the batch row or the packed sequence s) is read by the P·V MMA
+// V^T pad rule. Block s of m->vt ([max_batch][Hkv][128][Lpad], the batch row or the packed sequence s) is read by the P·V MMA
 // up to its padded length, and its columns [L_s, Lpad) meet P == 0 there: they must be finite zeros. A forward over blocks
 // [0, n) with lengths lens[] at column stride Lpad zeroes the whole buffer when the stride changes or when one of its blocks
 // holds columns beyond its new length (a longer forward wrote them); otherwise every column it reads past L_s is still zero.
@@ -590,7 +637,7 @@ static int vt_prepare(mmdp_model* m, int n, const int* lens, int Lpad, cudaStrea
     bool zero = m->vt_Lpad != Lpad;
     for (int i = 0; i < n && !zero; ++i) zero = m->vt_len[i] > lens[i];
     if (zero) {
-        MMDP_CUDA(cudaMemsetAsync(m->vt, 0, (size_t)m->cfg.max_batch * m->cfg.d_model * m->Lpad_max * 2, s));
+        MMDP_CUDA(cudaMemsetAsync(m->vt, 0, (size_t)m->cfg.max_batch * m->d_kv() * m->Lpad_max * 2, s));
         m->vt_len.assign(m->cfg.max_batch, 0);
         m->vt_Lpad = Lpad;
     }
@@ -631,7 +678,7 @@ static int model_forward(mmdp_model* m, const int64_t* ids, int B, int L, uint16
     if (n_b > 0 && (col0_b < 0 || ncols_b <= 0 || col0_b + ncols_b > c.vocab_size || (ncols_b % 8)))
         return set_error("mmdp_model_forward: bad column window [%d,+%d)", col0_b, ncols_b);
     cudaStream_t s = (cudaStream_t)stream;
-    const int d = c.d_model, ff = c.mlp_hidden, V = c.vocab_size, H = c.n_heads;
+    const int d = c.d_model, ff = c.mlp_hidden, V = c.vocab_size, H = c.n_heads, Hkv = m->n_kv_heads, dkv = m->d_kv();
     const int M = B * L;
     const int Lpad = ((L + 7) / 8) * 8;
     const std::vector<int> lens(B, L);
@@ -639,6 +686,8 @@ static int model_forward(mmdp_model* m, const int64_t* ids, int B, int L, uint16
     const float scale = 1.0f / sqrtf(128.0f);
     if (embed_rows(ids, m->wte, m->x, M, d, V, s, m->err_flag)) return -1;
     QkvRopeArgs qa{m->q, m->k, m->vt, m->cos_tab, m->sin_tab, L, Lpad, d, H};
+    qa.n_kv_heads = Hkv;
+    const int qkv_epi = m->gqa() ? EPI_QKVGQA : EPI_QKVROPE;
     // Row window of the LAST block: nothing after the last block mixes rows (ln_f and the LM head are row-wise and only the rows in
     // rows_a / rows_b are read), so its query rows / attn_out / MLP outside positions [row_lo, row_hi) of every batch row are dead
     // work: the keys and values of ALL rows are still computed, the rest of the block runs on the window only (per batch row).
@@ -647,10 +696,11 @@ static int model_forward(mmdp_model* m, const int64_t* ids, int B, int L, uint16
     for (int li = 0; li < c.n_layers; ++li) {
         const LayerWeights& l = m->layers[li];
         const bool win = window && li == c.n_layers - 1;
+        qa.bias = l.qkv_bias;
         if (rmsnorm(m->x, d, l.attn_norm, m->xn, d, M, d, c.rms_eps, s)) return -1;
-        if (block_linear(m, l, LIN_QKV, EPI_QKVROPE, m->xn, d, M, nullptr, 0, nullptr, 0, &qa, s)) return -1;
+        if (block_linear(m, l, LIN_QKV, qkv_epi, m->xn, d, M, nullptr, 0, nullptr, 0, &qa, s)) return -1;
         if (!win) {
-            if (attention_fwd(m->q, m->k, m->vt, m->att, B, H, L, Lpad, scale, s)) return -1;
+            if (attention_fwd(m->q, m->k, m->vt, m->att, B, H, L, Lpad, scale, s, 0, Hkv)) return -1;
             if (block_linear(m, l, LIN_O, EPI_RESID, m->att, d, M, m->x, d, m->x, d, nullptr, s)) return -1;
             if (rmsnorm(m->x, d, l.ff_norm, m->xn, d, M, d, c.rms_eps, s)) return -1;
             if (block_linear(m, l, LIN_13, EPI_SWIGLU, m->xn, d, M, m->h, ff, nullptr, 0, nullptr, s)) return -1;
@@ -660,7 +710,8 @@ static int model_forward(mmdp_model* m, const int64_t* ids, int B, int L, uint16
         const int Mw = row_hi - row_lo;
         for (int b = 0; b < B; ++b) {  // one row range per batch row (B = 1, or the CFG batch of variant M)
             const size_t r0 = (size_t)b * L + row_lo, o_d = r0 * d, o_ff = r0 * ff;
-            if (attention_fwd(m->q + o_d, m->k + (size_t)b * L * d, m->vt + (size_t)b * H * 128 * Lpad, m->att + o_d, 1, H, L, Lpad, scale, s, Mw)) return -1;
+            if (attention_fwd(m->q + o_d, m->k + (size_t)b * L * dkv, m->vt + (size_t)b * Hkv * 128 * Lpad, m->att + o_d, 1, H, L, Lpad, scale, s, Mw,
+                              Hkv)) return -1;
             if (block_linear(m, l, LIN_O, EPI_RESID, m->att + o_d, d, Mw, m->x + o_d, d, m->x + o_d, d, nullptr, s)) return -1;
             if (rmsnorm(m->x + o_d, d, l.ff_norm, m->xn + o_d, d, Mw, d, c.rms_eps, s)) return -1;
             if (block_linear(m, l, LIN_13, EPI_SWIGLU, m->xn + o_d, d, Mw, m->h + o_ff, ff, nullptr, 0, nullptr, s)) return -1;
@@ -718,7 +769,7 @@ MMDP_API int mmdp_model_forward_packed(mmdp_model* m, const int64_t* ids, int n_
     if (n_b > 0 && (col0_b < 0 || ncols_b <= 0 || col0_b + ncols_b > c.vocab_size || (ncols_b % 8)))
         return set_error("mmdp_model_forward_packed: bad column window [%d,+%d)", col0_b, ncols_b);
     cudaStream_t s = (cudaStream_t)stream;
-    const int d = c.d_model, ff = c.mlp_hidden, V = c.vocab_size, H = c.n_heads;
+    const int d = c.d_model, ff = c.mlp_hidden, V = c.vocab_size, H = c.n_heads, Hkv = m->n_kv_heads;
     const int M = segs.start[n_seg];
     const int Lpad = ((Lmax + 7) / 8) * 8;
     if (vt_prepare(m, n_seg, seg_len, Lpad, s)) return -1;
@@ -727,11 +778,14 @@ MMDP_API int mmdp_model_forward_packed(mmdp_model* m, const int64_t* ids, int n_
     if (embed_rows(ids, m->wte, m->x, M, d, V, s, m->err_flag)) return -1;
     QkvRopeArgs qa{m->q, m->k, m->vt, m->cos_tab, m->sin_tab, Lmax, Lpad, d, H};
     qa.seg_pos = m->seg_pos;
+    qa.n_kv_heads = Hkv;
+    const int qkv_epi = m->gqa() ? EPI_QKVGQA_PACKED : EPI_QKVROPE_PACKED;
     for (int li = 0; li < c.n_layers; ++li) {
         const LayerWeights& l = m->layers[li];
+        qa.bias = l.qkv_bias;
         if (rmsnorm(m->x, d, l.attn_norm, m->xn, d, M, d, c.rms_eps, s)) return -1;
-        if (block_linear(m, l, LIN_QKV, EPI_QKVROPE_PACKED, m->xn, d, M, nullptr, 0, nullptr, 0, &qa, s)) return -1;
-        if (attention_packed_fwd(m->q, m->k, m->vt, m->att, segs, H, Lpad, scale, s)) return -1;
+        if (block_linear(m, l, LIN_QKV, qkv_epi, m->xn, d, M, nullptr, 0, nullptr, 0, &qa, s)) return -1;
+        if (attention_packed_fwd(m->q, m->k, m->vt, m->att, segs, H, Lpad, scale, s, Hkv)) return -1;
         if (block_linear(m, l, LIN_O, EPI_RESID, m->att, d, M, m->x, d, m->x, d, nullptr, s)) return -1;
         if (rmsnorm(m->x, d, l.ff_norm, m->xn, d, M, d, c.rms_eps, s)) return -1;
         if (block_linear(m, l, LIN_13, EPI_SWIGLU, m->xn, d, M, m->h, ff, nullptr, 0, nullptr, s)) return -1;
@@ -747,6 +801,7 @@ MMDP_API int mmdp_model_forward_cached(mmdp_model* m, const int64_t* ids, int B,
     if (B <= 0 || B > c.max_batch || L <= 0 || L > c.max_seq_len || Tq <= 0 || Tq > L)
         return set_error("mmdp_model_forward_cached: B=%d L=%d Tq=%d outside workspace (max_batch=%d max_seq_len=%d)", B, L, Tq, c.max_batch, c.max_seq_len);
     if (!pos_map && Tq != L) return set_error("mmdp_model_forward_cached: a partial forward needs the position map");
+    if (m->gqa()) return set_error("mmdp_model_forward_cached: the token cache holds d_model-wide multi-head keys without a q/k/v bias");
     if (L > m->rope_len) return set_error("mmdp_model_forward_cached: rotary table covers %d positions, need %d", m->rope_len, L);
     cudaStream_t s = (cudaStream_t)stream;
     const int d = c.d_model, ff = c.mlp_hidden, V = c.vocab_size, H = c.n_heads;

@@ -7,7 +7,9 @@
 //     operand of O += P V (wgmma with A from registers, B = V^T from shared memory); O stays in registers for the whole loop;
 //   * the tiles of a partial last wave are cut along the keys and merged by attention_combine_kernel (see attention_fwd);
 //   * attention_packed_kernel runs the same body over a packed variable-length batch: work items enumerate
-//     (sequence, head, query tile), each sequence attends to its own keys only (attention_packed_fwd).
+//     (sequence, head, query tile), each sequence attends to its own keys only (attention_packed_fwd);
+//   * grouped-query attention (kGqa): query head h reads kv head h / kv_group of k [rows, 128 Hkv] and V^T [B][Hkv][128][Lpad];
+//     separate kernels, so that the multi-head ones keep their code.
 #include "mmdp_internal.h"
 #include "ptx.cuh"
 
@@ -45,10 +47,12 @@ struct AttnSegs {
 
 // One CTA's work item. kPacked = false: B sequences of L keys / Lq queries each, laid out batch row after batch row (the
 // kernel parameters). kPacked = true: the sequences of `segs`, each with its own length (L = Lq = its length).
-template <int kBKV, bool kPacked>
+// kGqa: H / kv_group kv heads, query head h reads kv head h / kv_group.
+template <int kBKV, bool kPacked, bool kGqa = false>
 __device__ __forceinline__ void attention_body(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmVt,
                                                __nv_bfloat16* __restrict__ out, int H, int L, int d_model, float scale_log2,
-                                               int n_full, int splits, float* __restrict__ part_ws, int Lq, const AttnSegs* segs) {
+                                               int n_full, int splits, float* __restrict__ part_ws, int Lq, const AttnSegs* segs,
+                                               int kv_group = 1) {
     constexpr int kKBytes = AttnCfg<kBKV>::kKBytes, kVBytes = AttnCfg<kBKV>::kVBytes;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -88,6 +92,7 @@ __device__ __forceinline__ void attention_body(const CUtensorMap& tmQ, const CUt
         tl = tile - segs->tile0[seg];
     }
     const int qt = tl % n_qt, h = (tl / n_qt) % H, b = kPacked ? seg : tile / (n_qt * H);
+    const int hk = kGqa ? h / kv_group : h, Hk = kGqa ? H / kv_group : H;  // kv head and kv head count
     int jb = 0, je = n_kv_all;
     if (piece >= 0) {
         const int per = (n_kv_all + splits - 1) / splits;
@@ -127,12 +132,12 @@ __device__ __forceinline__ void attention_body(const CUtensorMap& tmQ, const CUt
                 const int kv0 = (jb + j) * kBKV;
                 mbar_wait(&k_empty[st], ph ^ 1);
                 mbar_expect_tx(&k_full[st], kKBytes);
-                tma_load_2d(sK + st * kKBytes, &tmK, &k_full[st], h * 128, (kPacked ? seg0 : b * L) + kv0);
-                tma_load_2d(sK + st * kKBytes + kKBytes / 2, &tmK, &k_full[st], h * 128 + 64, (kPacked ? seg0 : b * L) + kv0);
+                tma_load_2d(sK + st * kKBytes, &tmK, &k_full[st], hk * 128, (kPacked ? seg0 : b * L) + kv0);
+                tma_load_2d(sK + st * kKBytes + kKBytes / 2, &tmK, &k_full[st], hk * 128 + 64, (kPacked ? seg0 : b * L) + kv0);
                 mbar_wait(&v_empty[st], ph ^ 1);
                 mbar_expect_tx(&v_full[st], kVBytes);
-                tma_load_2d(sV + st * kVBytes, &tmVt, &v_full[st], kv0, (b * H + h) * 128);
-                if (kBKV == 128) tma_load_2d(sV + st * kVBytes + kVBytes / 2, &tmVt, &v_full[st], kv0 + 64, (b * H + h) * 128);
+                tma_load_2d(sV + st * kVBytes, &tmVt, &v_full[st], kv0, (b * Hk + hk) * 128);
+                if (kBKV == 128) tma_load_2d(sV + st * kVBytes + kVBytes / 2, &tmVt, &v_full[st], kv0 + 64, (b * Hk + hk) * 128);
             }
         }
         __syncwarp();
@@ -272,6 +277,23 @@ attention_packed_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
     attention_body<kBKV, true>(tmQ, tmK, tmVt, out, H, 0, d_model, scale_log2, n_full, splits, part_ws, 0, &segs);
 }
 
+template <int kBKV>
+__global__ void __launch_bounds__(kAttnThreads, 1)
+attention_gqa_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                     const __grid_constant__ CUtensorMap tmVt, __nv_bfloat16* __restrict__ out, int H, int L, int d_model,
+                     float scale_log2, int n_full, int splits, float* __restrict__ part_ws, int Lq, int kv_group) {
+    attention_body<kBKV, false, true>(tmQ, tmK, tmVt, out, H, L, d_model, scale_log2, n_full, splits, part_ws, Lq, nullptr, kv_group);
+}
+
+template <int kBKV>
+__global__ void __launch_bounds__(kAttnThreads, 1)
+attention_packed_gqa_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                            const __grid_constant__ CUtensorMap tmVt, __nv_bfloat16* __restrict__ out, int H, int d_model,
+                            float scale_log2, int n_full, int splits, float* __restrict__ part_ws, const __grid_constant__ AttnSegs segs,
+                            int kv_group) {
+    attention_body<kBKV, true, true>(tmQ, tmK, tmVt, out, H, 0, d_model, scale_log2, n_full, splits, part_ws, 0, &segs, kv_group);
+}
+
 // Merges the `splits` KV-slice partials of one split tile: out = (sum_i w_i O_i) / (sum_i w_i l_i), w_i = 2^((m_i - m) c).
 // One CTA per (split tile, query row), thread = output column.
 template <bool kPacked>
@@ -385,16 +407,18 @@ static int attn_smem_attr(Kernel kernel, int smem, unsigned long long& attr_set)
 
 template <int kBKV>
 static int attention_launch(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* vt, __nv_bfloat16* out, int B, int H,
-                            int L, int Lpad, float scale, cudaStream_t stream, int Lq) {
+                            int L, int Lpad, float scale, cudaStream_t stream, int Lq, int Hkv) {
     constexpr int kAttnSmem = AttnCfg<kBKV>::kSmem;
     if (B <= 0 || H <= 0 || L <= 0) return set_error("attention: empty problem");
     if (Lq <= 0) Lq = L;
+    if (Hkv <= 0) Hkv = H;
+    if (Hkv > H || H % Hkv) return set_error("attention: n_kv_heads=%d must divide n_heads=%d", Hkv, H);
     if (Lpad < L || (Lpad % 8)) return set_error("attention: Lpad must be >= L and a multiple of 8");
-    const int d_model = H * 128;
+    const int d_model = H * 128, d_kv = Hkv * 128;
     CUtensorMap tmQ, tmK, tmVt;
     if (make_tmap_2d_bf16(&tmQ, q, (uint64_t)B * Lq, (uint64_t)d_model, (uint64_t)d_model, 128, 64)) return -1;
-    if (make_tmap_2d_bf16(&tmK, k, (uint64_t)B * L, (uint64_t)d_model, (uint64_t)d_model, kBKV, 64)) return -1;
-    if (make_tmap_2d_bf16(&tmVt, vt, (uint64_t)B * H * 128, (uint64_t)Lpad, (uint64_t)Lpad, 128, 64)) return -1;
+    if (make_tmap_2d_bf16(&tmK, k, (uint64_t)B * L, (uint64_t)d_kv, (uint64_t)d_kv, kBKV, 64)) return -1;
+    if (make_tmap_2d_bf16(&tmVt, vt, (uint64_t)B * Hkv * 128, (uint64_t)Lpad, (uint64_t)Lpad, 128, 64)) return -1;
     const int n_qt = (Lq + 127) / 128, n_kvb = (L + kBKV - 1) / kBKV;
     const int tiles = n_qt * H * B;
     int n_full, n_split, splits;
@@ -405,10 +429,17 @@ static int attention_launch(const __nv_bfloat16* q, const __nv_bfloat16* k, cons
     const float scale_log2 = scale * 1.4426950408889634f;
     const bool pdl = pdl_mode() != 0;
     LaunchScope ls(LK_ATTN, 4.0 * B * H * (double)Lq * L * 128, stream);
-    static unsigned long long attr_set = 0;
-    if (attn_smem_attr(attention_kernel<kBKV>, kAttnSmem, attr_set)) return -1;
-    MMDP_CUDA(launch_ex(attention_kernel<kBKV>, dim3(grid), dim3(kAttnThreads), kAttnSmem, stream, pdl, false, tmQ, tmK, tmVt, out, H, L,
-                        d_model, scale_log2, n_full, splits, part_ws, Lq));
+    if (Hkv != H) {
+        static unsigned long long attr_set_gqa = 0;
+        if (attn_smem_attr(attention_gqa_kernel<kBKV>, kAttnSmem, attr_set_gqa)) return -1;
+        MMDP_CUDA(launch_ex(attention_gqa_kernel<kBKV>, dim3(grid), dim3(kAttnThreads), kAttnSmem, stream, pdl, false, tmQ, tmK, tmVt, out,
+                            H, L, d_model, scale_log2, n_full, splits, part_ws, Lq, H / Hkv));
+    } else {
+        static unsigned long long attr_set = 0;
+        if (attn_smem_attr(attention_kernel<kBKV>, kAttnSmem, attr_set)) return -1;
+        MMDP_CUDA(launch_ex(attention_kernel<kBKV>, dim3(grid), dim3(kAttnThreads), kAttnSmem, stream, pdl, false, tmQ, tmK, tmVt, out, H, L,
+                            d_model, scale_log2, n_full, splits, part_ws, Lq));
+    }
     if (n_split > 0)
         MMDP_CUDA(launch_ex(attention_combine_kernel, dim3(n_split, 128), dim3(128), 0, stream, pdl, false, (const float*)part_ws, out, H, Lq,
                             d_model, scale_log2, n_full, splits));
@@ -417,9 +448,11 @@ static int attention_launch(const __nv_bfloat16* q, const __nv_bfloat16* k, cons
 
 template <int kBKV>
 static int attention_packed_launch(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* vt, __nv_bfloat16* out,
-                                   const SegTable& segs, int H, int Lpad, float scale, cudaStream_t stream) {
+                                   const SegTable& segs, int H, int Lpad, float scale, cudaStream_t stream, int Hkv) {
     constexpr int kAttnSmem = AttnCfg<kBKV>::kSmem;
     if (segs.n <= 0 || segs.n > kMaxSegs || H <= 0) return set_error("attention_packed: %d sequences (1 to %d)", segs.n, kMaxSegs);
+    if (Hkv <= 0) Hkv = H;
+    if (Hkv > H || H % Hkv) return set_error("attention_packed: n_kv_heads=%d must divide n_heads=%d", Hkv, H);
     if (Lpad % 8) return set_error("attention_packed: Lpad must be a multiple of 8");
     AttnSegs as{};
     as.n = segs.n;
@@ -432,11 +465,11 @@ static int attention_packed_launch(const __nv_bfloat16* q, const __nv_bfloat16* 
         as.tile0[s + 1] = as.tile0[s] + (len + 127) / 128 * H;
         work += 4.0 * H * (double)len * len * 128;
     }
-    const int M = segs.start[segs.n], tiles = as.tile0[segs.n], d_model = H * 128;
+    const int M = segs.start[segs.n], tiles = as.tile0[segs.n], d_model = H * 128, d_kv = Hkv * 128;
     CUtensorMap tmQ, tmK, tmVt;
     if (make_tmap_2d_bf16(&tmQ, q, (uint64_t)M, (uint64_t)d_model, (uint64_t)d_model, 128, 64)) return -1;
-    if (make_tmap_2d_bf16(&tmK, k, (uint64_t)M, (uint64_t)d_model, (uint64_t)d_model, kBKV, 64)) return -1;
-    if (make_tmap_2d_bf16(&tmVt, vt, (uint64_t)segs.n * H * 128, (uint64_t)Lpad, (uint64_t)Lpad, 128, 64)) return -1;
+    if (make_tmap_2d_bf16(&tmK, k, (uint64_t)M, (uint64_t)d_kv, (uint64_t)d_kv, kBKV, 64)) return -1;
+    if (make_tmap_2d_bf16(&tmVt, vt, (uint64_t)segs.n * Hkv * 128, (uint64_t)Lpad, (uint64_t)Lpad, 128, 64)) return -1;
     auto kvb_of = [&](int t) {
         int s = 0;
         while (s + 1 < segs.n && t >= as.tile0[s + 1]) ++s;
@@ -450,10 +483,17 @@ static int attention_packed_launch(const __nv_bfloat16* q, const __nv_bfloat16* 
     const float scale_log2 = scale * 1.4426950408889634f;
     const bool pdl = pdl_mode() != 0;
     LaunchScope ls(LK_ATTN, work, stream);
-    static unsigned long long attr_set = 0;
-    if (attn_smem_attr(attention_packed_kernel<kBKV>, kAttnSmem, attr_set)) return -1;
-    MMDP_CUDA(launch_ex(attention_packed_kernel<kBKV>, dim3(grid), dim3(kAttnThreads), kAttnSmem, stream, pdl, false, tmQ, tmK, tmVt, out,
-                        H, d_model, scale_log2, n_full, splits, part_ws, as));
+    if (Hkv != H) {
+        static unsigned long long attr_set_gqa = 0;
+        if (attn_smem_attr(attention_packed_gqa_kernel<kBKV>, kAttnSmem, attr_set_gqa)) return -1;
+        MMDP_CUDA(launch_ex(attention_packed_gqa_kernel<kBKV>, dim3(grid), dim3(kAttnThreads), kAttnSmem, stream, pdl, false, tmQ, tmK, tmVt,
+                            out, H, d_model, scale_log2, n_full, splits, part_ws, as, H / Hkv));
+    } else {
+        static unsigned long long attr_set = 0;
+        if (attn_smem_attr(attention_packed_kernel<kBKV>, kAttnSmem, attr_set)) return -1;
+        MMDP_CUDA(launch_ex(attention_packed_kernel<kBKV>, dim3(grid), dim3(kAttnThreads), kAttnSmem, stream, pdl, false, tmQ, tmK, tmVt, out,
+                            H, d_model, scale_log2, n_full, splits, part_ws, as));
+    }
     if (n_split > 0)
         MMDP_CUDA(launch_ex(attention_packed_combine_kernel, dim3(n_split, 128), dim3(128), 0, stream, pdl, false, (const float*)part_ws,
                             out, H, d_model, scale_log2, n_full, splits, as));
@@ -461,19 +501,19 @@ static int attention_packed_launch(const __nv_bfloat16* q, const __nv_bfloat16* 
 }
 
 int attention_fwd(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* vt, __nv_bfloat16* out, int B, int H, int L,
-                  int Lpad, float scale, cudaStream_t stream, int Lq) {
+                  int Lpad, float scale, cudaStream_t stream, int Lq, int Hkv) {
     const int version = opt(OPT_ATTN_VERSION);
-    if (version == 7) return attention_launch<64>(q, k, vt, out, B, H, L, Lpad, scale, stream, Lq);
+    if (version == 7) return attention_launch<64>(q, k, vt, out, B, H, L, Lpad, scale, stream, Lq, Hkv);
     if (version != 6) return set_error("attention: unknown kernel generation %d (6 or 7)", version);
-    return attention_launch<128>(q, k, vt, out, B, H, L, Lpad, scale, stream, Lq);
+    return attention_launch<128>(q, k, vt, out, B, H, L, Lpad, scale, stream, Lq, Hkv);
 }
 
 int attention_packed_fwd(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* vt, __nv_bfloat16* out,
-                         const SegTable& segs, int H, int Lpad, float scale, cudaStream_t stream) {
+                         const SegTable& segs, int H, int Lpad, float scale, cudaStream_t stream, int Hkv) {
     const int version = opt(OPT_ATTN_VERSION);
-    if (version == 7) return attention_packed_launch<64>(q, k, vt, out, segs, H, Lpad, scale, stream);
+    if (version == 7) return attention_packed_launch<64>(q, k, vt, out, segs, H, Lpad, scale, stream, Hkv);
     if (version != 6) return set_error("attention: unknown kernel generation %d (6 or 7)", version);
-    return attention_packed_launch<128>(q, k, vt, out, segs, H, Lpad, scale, stream);
+    return attention_packed_launch<128>(q, k, vt, out, segs, H, Lpad, scale, stream, Hkv);
 }
 
 }  // namespace mmdp

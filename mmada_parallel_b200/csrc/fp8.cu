@@ -245,6 +245,10 @@ int gemm_fp8(int epi, const uint8_t* A, int lda, const float* sa, const uint8_t*
             if (epi == EPI_QKVROPE_PACKED ? !qa->seg_pos : (qa->pos_map ? (qa->Tq <= 0 || M % qa->Tq) : (!qa->chunked && (M % qa->L))))
                 return set_error("gemm_fp8: qkv epilogue needs M == B*L (or B*Tq with a position map, or a packed row map)");
             break;
+        case EPI_QKVGQA:
+        case EPI_QKVGQA_PACKED:
+            if (qkv_gqa_check("gemm_fp8", epi, M, N, qa)) return -1;
+            break;
         default:
             return set_error("gemm_fp8: unsupported epilogue %d", epi);
     }
@@ -256,6 +260,7 @@ int gemm_fp8(int epi, const uint8_t* A, int lda, const float* sa, const uint8_t*
         p.q = qa->q; p.k = qa->k; p.vt = qa->vt; p.cos_tab = qa->cos_tab; p.sin_tab = qa->sin_tab;
         p.L = qa->L; p.Lpad = qa->Lpad; p.d_model = qa->d_model; p.n_heads = qa->n_heads;
         p.pos_map = qa->pos_map; p.Tq = qa->Tq; p.row0 = qa->row0; p.seg_pos = qa->seg_pos;
+        p.n_kv_heads = qa->n_kv_heads; p.bias = qa->bias;
     }
     const Fp8Scales sc{sa, sw};
     const int tiles = ((M + kF8BM - 1) / kF8BM) * ((N + kF8BN - 1) / kF8BN);
@@ -268,6 +273,8 @@ int gemm_fp8(int epi, const uint8_t* A, int lda, const float* sa, const uint8_t*
         case EPI_RESID: return launch_gemm_fp8<EPI_RESID>(tmA, tmB, p, sc, grid, stream);
         case EPI_SWIGLU: return launch_gemm_fp8<EPI_SWIGLU>(tmA, tmB, p, sc, grid, stream);
         case EPI_QKVROPE_PACKED: return launch_gemm_fp8<EPI_QKVROPE_PACKED>(tmA, tmB, p, sc, grid, stream);
+        case EPI_QKVGQA: return launch_gemm_fp8<EPI_QKVGQA>(tmA, tmB, p, sc, grid, stream);
+        case EPI_QKVGQA_PACKED: return launch_gemm_fp8<EPI_QKVGQA_PACKED>(tmA, tmB, p, sc, grid, stream);
         default: return launch_gemm_fp8<EPI_QKVROPE>(tmA, tmB, p, sc, grid, stream);
     }
 }

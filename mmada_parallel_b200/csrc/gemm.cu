@@ -14,6 +14,7 @@
 //   EPI_QKVROPE : q,k = bf16( rope_fp32( bf16(acc) ) ), v^T = bf16(acc)    (q/k/v_proj :925-927 + RotaryEmbedding :402-435)
 //   EPI_SWIGLU  : C = bf16( bf16(silu(bf16(g))) * bf16(u) )                (ff_proj/up_proj/act/mul :962-967)
 //   EPI_QKVROPE_PACKED : EPI_QKVROPE over a packed variable-length batch (per-row sequence and position)
+//   EPI_QKVGQA(_PACKED): the two above with grouped-query k / v and q,k,v = bf16(acc + bias)   (k/v_proj :872-884)
 #include "gemm_epilogue.cuh"
 
 #include <stdlib.h>
@@ -66,13 +67,14 @@ __device__ __forceinline__ void bf16x8_to_float(uint4 x, float (&f)[8]) {
 // V^T of a staged QKV tile: items are 8 rows x 8 columns. When the 8 rows are 8 consecutive positions of one sequence starting
 // at a multiple of 8, the block is transposed in registers and each column (one d of V^T) is one 16-byte store; otherwise
 // (a sequence boundary inside the 8 rows, a position map, rows past M) every row goes through epi_row8's element stores.
+// Grouped-query tiles (EPI_QKVGQA*) pass cg0 = 16 x the tile's rotary halves: only the 8-column groups from cg0 on are V.
 template <int EPI, int BN>
-__device__ __forceinline__ void staged_vt(const GemmParams& p, const uint8_t* stg, int m_blk, int n_blk, int etid) {
+__device__ __forceinline__ void staged_vt(const GemmParams& p, const uint8_t* stg, int m_blk, int n_blk, int etid, int cg0 = 0) {
     constexpr int kStride = GemmCfg<BN, true>::kStagingStride;
-    constexpr int CG = BN / 8;
+    const int CG = BN / 8 - cg0;
     const bool aligned = (p.Lpad & 7) == 0 && (reinterpret_cast<uintptr_t>(p.vt) & 15) == 0;
     for (int idx = etid; idx < 16 * CG; idx += kStagedEpiThreads) {
-        const int rg = idx / CG, cg = idx - rg * CG;
+        const int rg = idx / CG, cg = cg0 + idx - rg * CG;
         const int r0 = m_blk * 128 + 8 * rg;
         if (r0 >= p.M) continue;
         uint4 x[8];
@@ -87,9 +89,9 @@ __device__ __forceinline__ void staged_vt(const GemmParams& p, const uint8_t* st
             vec = b == b0 && pos == pos0 + i;
         }
         if (vec) {
-            const int n = n_blk * BN - 2 * p.d_model + 8 * cg;
+            const int n = n_blk * BN - (epi_is_gqa(EPI) ? p.d_model + p.n_kv_heads * 128 : 2 * p.d_model) + 8 * cg;
             const int head = n >> 7, d0 = n & 127;
-            __nv_bfloat16* dst = p.vt + ((size_t)(b0 * p.n_heads + head) * 128 + d0) * p.Lpad + pos0;
+            __nv_bfloat16* dst = p.vt + ((size_t)(b0 * (epi_is_gqa(EPI) ? p.n_kv_heads : p.n_heads) + head) * 128 + d0) * p.Lpad + pos0;
 #pragma unroll
             for (int c = 0; c < 8; ++c) {
                 uint32_t o[4];
@@ -128,9 +130,16 @@ __device__ __forceinline__ void staged_epilogue(const GemmParams& p, const uint8
             return;
         }
     }
-    constexpr bool kPair = EPI == EPI_SWIGLU || EPI == EPI_QKVROPE || EPI == EPI_QKVROPE_PACKED;
+    // grouped-query tiles: V halves through staged_vt, then the rotary items of the q / k halves (8 per half and row)
+    int n_rot = BN / 128;
+    if constexpr (epi_is_gqa(EPI)) {
+        n_rot = gqa_rot_halves<BN>(p, n_blk);
+        if (n_rot < BN / 128) staged_vt<EPI, BN>(p, stg, m_blk, n_blk, etid, 16 * n_rot);
+    }
+    constexpr bool kPair = EPI == EPI_SWIGLU || epi_is_qkv(EPI);
     constexpr int G = kPair ? 16 : BN / 8;
-    constexpr int kItems = BM * G;
+    const int kItems = epi_is_gqa(EPI) ? BM * 8 * n_rot : BM * G;
+    const int Gi = epi_is_gqa(EPI) ? 8 * n_rot : G;
     constexpr int U = kPair ? 1 : 4;
     for (int i0 = etid; i0 < kItems; i0 += U * kStagedEpiThreads) {
         uint4 xv[U], xw[U], rv[U];
@@ -138,7 +147,7 @@ __device__ __forceinline__ void staged_epilogue(const GemmParams& p, const uint8
 #pragma unroll
         for (int u = 0; u < U; ++u) {
             const int idx = i0 + u * kStagedEpiThreads;
-            const int rit = idx / G, g = idx - rit * G;
+            const int rit = idx / Gi, g = idx - rit * Gi;
             // SwiGLU g -> gate columns 8g, up +128; rotary g = (head, gg) -> 128 head + 8 gg, partner +64
             tc[u] = EPI == EPI_SWIGLU ? 8 * g : (kPair ? (g >> 3) * 128 + 8 * (g & 7) : 8 * g);
             row[u] = (idx < kItems && m_blk * BM + rit < p.M) ? m_blk * BM + rit : -1;
@@ -329,6 +338,18 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             if constexpr (kStaged) {
                 // the previous tile has left the staging tile a whole main loop ago; the epilogue warps apply the fused
                 // epilogue while this warpgroup runs the next tile's k-blocks
+                if constexpr (epi_is_gqa(EPI)) {  // the bias joins the fp32 accumulator before the one bf16 rounding
+                    if (p.bias) {
+#pragma unroll
+                        for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                const float bv = __bfloat162float(p.bias[n_blk * BN + 8 * j + c0 + e]);
+                                acc[4 * j + e] = __fadd_rn(acc[4 * j + e], bv);
+                                acc[4 * j + 2 + e] = __fadd_rn(acc[4 * j + 2 + e], bv);
+                            }
+                    }
+                }
                 mbar_wait(drained_bar, (it & 1) ^ 1);
                 stage_tile<BN>(staging, acc, rit0, c0);
                 mbar_arrive(staged_bar);
@@ -627,6 +648,10 @@ int gemm_bf16(int epi, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, 
             if (epi == EPI_QKVROPE_PACKED ? !qa->seg_pos : (qa->pos_map ? (qa->Tq <= 0 || M % qa->Tq) : (!qa->chunked && (M % qa->L))))
                 return set_error("gemm: qkv epilogue needs M == B*L (or B*Tq with a position map, or a packed row map)");
             break;
+        case EPI_QKVGQA:
+        case EPI_QKVGQA_PACKED:
+            if (qkv_gqa_check("gemm", epi, M, N, qa)) return -1;
+            break;
         default:
             return set_error("gemm: unknown epilogue");
     }
@@ -655,6 +680,7 @@ int gemm_bf16(int epi, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, 
         p.q = qa->q; p.k = qa->k; p.vt = qa->vt; p.cos_tab = qa->cos_tab; p.sin_tab = qa->sin_tab;
         p.L = qa->L; p.Lpad = qa->Lpad; p.d_model = qa->d_model; p.n_heads = qa->n_heads;
         p.pos_map = qa->pos_map; p.Tq = qa->Tq; p.row0 = qa->row0; p.seg_pos = qa->seg_pos;
+        p.n_kv_heads = qa->n_kv_heads; p.bias = qa->bias;
     }
     // kernel selection: MMDP_GEMM_PAIR / mmdp_set_gemm_pair 0 (default) = one CTA per tile (with the split-K tail), 1 = CTA
     // pairs for M > 256, 2 = pairs only for M >= 4096 and N >= 8192
@@ -672,6 +698,8 @@ int gemm_bf16(int epi, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, 
             case EPI_SWIGLU: return launch_gemm_pair<EPI_SWIGLU, 256>(tmA, tmBh, p, pair_tiles, stream);
             case EPI_QKVROPE: return launch_gemm_pair<EPI_QKVROPE, 256>(tmA, tmBh, p, pair_tiles, stream);
             case EPI_QKVROPE_PACKED: return launch_gemm_pair<EPI_QKVROPE_PACKED, 256>(tmA, tmBh, p, pair_tiles, stream);
+            case EPI_QKVGQA: return launch_gemm_pair<EPI_QKVGQA, 256>(tmA, tmBh, p, pair_tiles, stream);
+            case EPI_QKVGQA_PACKED: return launch_gemm_pair<EPI_QKVGQA_PACKED, 256>(tmA, tmBh, p, pair_tiles, stream);
             default: return set_error("gemm: unknown epilogue");
         }
     }
@@ -701,6 +729,10 @@ int gemm_bf16(int epi, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, 
             return launch_gemm<EPI_QKVROPE, 256>(tmA, tmB, p, grid, stream);
         case EPI_QKVROPE_PACKED:
             return launch_gemm<EPI_QKVROPE_PACKED, 256>(tmA, tmB, p, grid, stream);
+        case EPI_QKVGQA:
+            return launch_gemm<EPI_QKVGQA, 256>(tmA, tmB, p, grid, stream);
+        case EPI_QKVGQA_PACKED:
+            return launch_gemm<EPI_QKVGQA_PACKED, 256>(tmA, tmB, p, grid, stream);
         default:
             return set_error("gemm: unknown epilogue");
     }

@@ -46,7 +46,24 @@ struct GemmParams {
     // EPI_QKVROPE_PACKED: (sequence, position) of every row of a packed variable-length batch; q / k stay at the row,
     // v^T goes to vt[sequence][head][d][position]
     const int2* seg_pos;
+    // EPI_QKVGQA*: kv heads (k is [M, 128 n_kv_heads], v^T [B][n_kv_heads][128][Lpad]) and the q | k | v bias (nullable)
+    int n_kv_heads;
+    const __nv_bfloat16* bias;
 };
+
+// Host-side argument check of the grouped-query QKV epilogues (bf16 and e4m3 GEMM). The token-cache and row-chunked
+// launches stay on the multi-head epilogue.
+inline int qkv_gqa_check(const char* who, int epi, int M, int N, const QkvRopeArgs* qa) {
+    if (!qa) return set_error("%s: qkv epilogue needs QkvRopeArgs", who);
+    const int d = qa->d_model, H = qa->n_heads, Hkv = qa->n_kv_heads;
+    if (d % 256 || d != H * 128) return set_error("%s: qkv epilogue needs head_dim 128 and d_model %% 256 == 0", who);
+    if (Hkv <= 0 || Hkv > H || H % Hkv) return set_error("%s: n_kv_heads=%d must divide n_heads=%d", who, Hkv, H);
+    if (N != d + 2 * 128 * Hkv) return set_error("%s: grouped-query qkv needs N == d_model + 2 * 128 * n_kv_heads", who);
+    if (qa->pos_map || qa->chunked || qa->row0) return set_error("%s: grouped-query qkv has no token-cache or row-chunked form", who);
+    if (epi == EPI_QKVGQA_PACKED ? !qa->seg_pos : (qa->L <= 0 || M % qa->L))
+        return set_error("%s: qkv epilogue needs M == B*L (or a packed row map)", who);
+    return 0;
+}
 
 __host__ __device__ __forceinline__ void gemm_tile_coords(int tl, int num_m, int num_n, int group_m, int& m_blk, int& n_blk) {
     if (group_m <= 0 || group_m >= num_m) {
@@ -60,6 +77,44 @@ __host__ __device__ __forceinline__ void gemm_tile_coords(int tl, int num_m, int
         m_blk = first + r % gsz;
         n_blk = r / gsz;
     }
+}
+
+// Row and (sequence, position) of GEMM row `row` for the QKV epilogues (the same mapping as gemm_epilogue_tile's).
+template <int EPI>
+__device__ __forceinline__ void qkv_row_coords(const GemmParams& p, int row, int& b, int& pos) {
+    if constexpr (epi_is_packed(EPI)) {
+        const int2 sp = p.seg_pos[row];
+        b = sp.x;
+        pos = sp.y;
+    } else if (p.pos_map) {
+        b = row / p.Tq;
+        pos = p.pos_map[row];
+    } else {
+        b = (row + p.row0) / p.L;
+        pos = (row + p.row0) - b * p.L;
+    }
+}
+
+// EPI_QKVGQA*: accumulator of GEMM column `col` plus its bias, in fp32 (nn.Linear rounds acc + bias to bf16 once)
+__device__ __forceinline__ float qkv_biased(const GemmParams& p, int col, float acc) {
+    return p.bias ? __fadd_rn(acc, __bfloat162float(p.bias[col])) : acc;
+}
+
+// EPI_QKVGQA*: the rotary pair (t1 at column c, t2 at c + 64 of a q / k head) and its two bf16 outputs, or a V^T element
+__device__ __forceinline__ void rope_pair(float t1, float t2, float cs, float sn, float& a, float& b) {
+    // (t * cos) + (rotate_half(t) * sin), fp32, no FMA contraction
+    a = __fadd_rn(__fmul_rn(t1, cs), __fmul_rn(-t2, sn));
+    b = __fadd_rn(__fmul_rn(t2, cs), __fmul_rn(t1, sn));
+}
+
+// EPI_QKVGQA*: destination of GEMM column `col` (a q / k head start + c, c < 64) of row `row`
+__device__ __forceinline__ __nv_bfloat16* gqa_qk_dst(const GemmParams& p, int row, int col) {
+    return col < p.d_model ? p.q + (size_t)row * p.d_model + col : p.k + (size_t)row * (p.n_kv_heads * 128) + (col - p.d_model);
+}
+// EPI_QKVGQA*: V^T element of GEMM column `col` (>= d + d_kv) for sequence b, position pos
+__device__ __forceinline__ __nv_bfloat16* gqa_vt_dst(const GemmParams& p, int col, int b, int pos) {
+    const int n = col - p.d_model - p.n_kv_heads * 128;
+    return p.vt + ((size_t)(b * p.n_kv_heads + (n >> 7)) * 128 + (n & 127)) * p.Lpad + pos;
 }
 
 // One thread's share of a 128 x BN accumulator tile (gemm.cu): the wgmma fragment of its warpgroup's 64-row half,
@@ -169,6 +224,42 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
                     dst[p.Lpad] = __float2bfloat16_rn(acc[4 * j + 2 * h + 1]);
                 }
             }
+        } else if constexpr (epi_is_gqa(EPI)) {
+            // q | k | v regions are 128-column aligned but a tile may straddle the k | v boundary: decided per head
+            int b, pos;
+            qkv_row_coords<EPI>(p, row, b, pos);
+#pragma unroll
+            for (int head = 0; head < BN / 128; ++head) {
+                const int col0 = n0 + head * 128;
+                if (col0 >= p.N) continue;
+                if (col0 < p.d_model + p.n_kv_heads * 128) {
+#pragma unroll
+                    for (int jj = 0; jj < 8; ++jj) {
+                        const int j = head * 16 + jj, c = 8 * jj + c0;
+                        const float2 cs = *reinterpret_cast<const float2*>(p.cos_tab + (size_t)pos * 64 + c);
+                        const float2 sn = *reinterpret_cast<const float2*>(p.sin_tab + (size_t)pos * 64 + c);
+                        const float csv[2] = {cs.x, cs.y}, snv[2] = {sn.x, sn.y};
+                        float a[2], bb[2];
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const float t1 = bf16_round(qkv_biased(p, col0 + c + e, acc[4 * j + 2 * h + e]));
+                            const float t2 = bf16_round(qkv_biased(p, col0 + 64 + c + e, acc[4 * (j + 8) + 2 * h + e]));
+                            rope_pair(t1, t2, csv[e], snv[e], a[e], bb[e]);
+                        }
+                        __nv_bfloat16* dst = gqa_qk_dst(p, row, col0 + c);
+                        *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(a[0], a[1]);
+                        *reinterpret_cast<uint32_t*>(dst + 64) = pack_bf16x2(bb[0], bb[1]);
+                    }
+                } else {
+#pragma unroll
+                    for (int jj = 0; jj < 16; ++jj) {
+                        const int j = head * 16 + jj, col = col0 + 8 * jj + c0;
+                        __nv_bfloat16* dst = gqa_vt_dst(p, col, b, pos);
+                        dst[0] = __float2bfloat16_rn(qkv_biased(p, col, acc[4 * j + 2 * h]));
+                        dst[p.Lpad] = __float2bfloat16_rn(qkv_biased(p, col + 1, acc[4 * j + 2 * h + 1]));
+                    }
+                }
+            }
         }
     }
 }
@@ -228,22 +319,6 @@ __device__ __forceinline__ void sk_publish(float* __restrict__ slot_ws, const fl
             *reinterpret_cast<float2*>(slot_ws + ((size_t)(col >> 2) * 128 + rit0 + 8 * h) * 4 + (col & 3)) =
                 make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
         }
-}
-
-// Row and (sequence, position) of GEMM row `row` for the QKV epilogues (the same mapping as gemm_epilogue_tile's).
-template <int EPI>
-__device__ __forceinline__ void qkv_row_coords(const GemmParams& p, int row, int& b, int& pos) {
-    if constexpr (EPI == EPI_QKVROPE_PACKED) {
-        const int2 sp = p.seg_pos[row];
-        b = sp.x;
-        pos = sp.y;
-    } else if (p.pos_map) {
-        b = row / p.Tq;
-        pos = p.pos_map[row];
-    } else {
-        b = (row + p.row0) / p.L;
-        pos = (row + p.row0) - b * p.L;
-    }
 }
 
 // One work item of the fused epilogue, shared by the split-K finishing pass (fp32 sums) and the staged epilogue of
@@ -321,7 +396,39 @@ __device__ __forceinline__ void epi_row8(const GemmParams& p, int row, int n_blk
 #pragma unroll
             for (int i = 0; i < 8; ++i) dst[(size_t)i * p.Lpad] = __float2bfloat16_rn(v[i]);
         }
+    } else if constexpr (epi_is_gqa(EPI)) {
+        // v / w already hold acc + bias (the caller adds it before any rounding)
+        int b, pos;
+        qkv_row_coords<EPI>(p, row, b, pos);
+        const int col = n0 + tc;
+        if (col < p.d_model + p.n_kv_heads * 128) {
+            const int c = tc & 63;
+            const float4* c4 = reinterpret_cast<const float4*>(p.cos_tab + (size_t)pos * 64 + c);
+            const float4* s4 = reinterpret_cast<const float4*>(p.sin_tab + (size_t)pos * 64 + c);
+            const float4 c0 = c4[0], c1 = c4[1], s0 = s4[0], s1 = s4[1];
+            const float cs[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
+            const float sn[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
+            float o1[8], o2[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) rope_pair(bf16_round(v[i]), bf16_round(w[i]), cs[i], sn[i], o1[i], o2[i]);
+            __nv_bfloat16* dst = gqa_qk_dst(p, row, col);
+            *reinterpret_cast<uint4*>(dst) =
+                make_uint4(pack_bf16x2(o1[0], o1[1]), pack_bf16x2(o1[2], o1[3]), pack_bf16x2(o1[4], o1[5]), pack_bf16x2(o1[6], o1[7]));
+            *reinterpret_cast<uint4*>(dst + 64) =
+                make_uint4(pack_bf16x2(o2[0], o2[1]), pack_bf16x2(o2[2], o2[3]), pack_bf16x2(o2[4], o2[5]), pack_bf16x2(o2[6], o2[7]));
+        } else {
+            __nv_bfloat16* dst = gqa_vt_dst(p, col, b, pos);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) dst[(size_t)i * p.Lpad] = __float2bfloat16_rn(v[i]);
+        }
     }
+}
+
+// EPI_QKVGQA*: number of leading 128-column halves of tile n_blk that are q / k (rotary); the rest are V
+template <int BN>
+__device__ __forceinline__ int gqa_rot_halves(const GemmParams& p, int n_blk) {
+    const int lim = p.d_model + p.n_kv_heads * 128 - n_blk * BN;
+    return lim <= 0 ? 0 : (lim >= BN ? BN / 128 : lim / 128);
 }
 
 template <int EPI, int BN>
@@ -329,6 +436,42 @@ __device__ __forceinline__ void sk_finish(const GemmParams& p, const float4* __r
                                           int n_blk, int tid) {
     const int r0 = (128 * unit_s) / S, r1 = (128 * (unit_s + 1)) / S;
     const int nrows = r1 - r0;
+    if constexpr (epi_is_gqa(EPI)) {
+        // per 128-column half: the rotary halves carry 8 paired items per row, the V halves 16 single ones
+        const int nrot = gqa_rot_halves<BN>(p, n_blk);
+        const int G = 8 * nrot + 16 * (BN / 128 - nrot);
+        for (int idx = tid; idx < nrows * G; idx += kEpiThreads) {
+            const int g = idx / nrows, rit = r0 + idx - g * nrows;
+            const int row = m_blk * 128 + rit;
+            if (row >= p.M) continue;
+            const bool rot = g < 8 * nrot;
+            const int tc = rot ? (g >> 3) * 128 + 8 * (g & 7) : 128 * nrot + 8 * (g - 8 * nrot);
+            const int col = n_blk * BN + tc;
+            if (col >= p.N) continue;
+            float v[8], w[8];
+            const int col4[4] = {tc / 4, tc / 4 + 1, (tc + 64) / 4, (tc + 64) / 4 + 1};
+            float4 a[4];
+            if (rot) sk_sum<BN, 4>(tile_ws, S, rit, col4, a);
+            else {
+                const int c2[2] = {col4[0], col4[1]};
+                float4 a2[2];
+                sk_sum<BN, 2>(tile_ws, S, rit, c2, a2);
+                a[0] = a2[0]; a[1] = a2[1]; a[2] = a[3] = make_float4(0.f, 0.f, 0.f, 0.f);
+            }
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                v[4 * i] = a[i].x; v[4 * i + 1] = a[i].y; v[4 * i + 2] = a[i].z; v[4 * i + 3] = a[i].w;
+                w[4 * i] = a[2 + i].x; w[4 * i + 1] = a[2 + i].y; w[4 * i + 2] = a[2 + i].z; w[4 * i + 3] = a[2 + i].w;
+            }
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                v[i] = qkv_biased(p, col + i, v[i]);
+                if (rot) w[i] = qkv_biased(p, col + 64 + i, w[i]);
+            }
+            epi_row8<EPI, BN>(p, row, n_blk, tc, v, w, make_uint4(0, 0, 0, 0));
+        }
+        return;
+    }
     // items per tile row: 8-column groups; the rotary (q / k) and SwiGLU items carry their partner columns
     const bool pair = EPI == EPI_SWIGLU || ((EPI == EPI_QKVROPE || EPI == EPI_QKVROPE_PACKED) && n_blk * BN < 2 * p.d_model);
     const int G = pair ? 16 : BN / 8;

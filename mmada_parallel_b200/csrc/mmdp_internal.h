@@ -9,7 +9,13 @@
 namespace mmdp {
 
 // EPI_QKVROPE_PACKED: EPI_QKVROPE over a packed variable-length batch (QkvRopeArgs::seg_pos)
-enum Epilogue { EPI_PLAIN = 0, EPI_RESID = 1, EPI_QKVROPE = 2, EPI_SWIGLU = 3, EPI_F32 = 4, EPI_QKVROPE_PACKED = 5 };
+// EPI_QKVGQA / EPI_QKVGQA_PACKED: the same two with grouped-query k / v (n_kv_heads <= n_heads) and an optional q / k / v bias;
+// the multi-head instantiations above stay free of both
+enum Epilogue { EPI_PLAIN = 0, EPI_RESID = 1, EPI_QKVROPE = 2, EPI_SWIGLU = 3, EPI_F32 = 4, EPI_QKVROPE_PACKED = 5,
+                EPI_QKVGQA = 6, EPI_QKVGQA_PACKED = 7 };
+constexpr bool epi_is_gqa(int epi) { return epi == EPI_QKVGQA || epi == EPI_QKVGQA_PACKED; }
+constexpr bool epi_is_qkv(int epi) { return epi == EPI_QKVROPE || epi == EPI_QKVROPE_PACKED || epi_is_gqa(epi); }
+constexpr bool epi_is_packed(int epi) { return epi == EPI_QKVROPE_PACKED || epi == EPI_QKVGQA_PACKED; }
 
 // Packed variable-length batch: sequence s occupies rows [start[s], start[s + 1]) of one packed row space; attention never
 // crosses from one sequence into another and positions restart at 0 in each. kMaxSegs bounds the sequences of one launch
@@ -123,6 +129,10 @@ struct QkvRopeArgs {
     int row0 = 0;  // GEMM row r is token row0 + r of the flattened [B*L] sequence (row-chunked tensor-parallel forward); q / k point at that row
     const int2* seg_pos = nullptr;  // EPI_QKVROPE_PACKED: row r is token seg_pos[r].y of sequence seg_pos[r].x (q / k stay at row r,
                                     // v^T goes to vt[seg][head][d][pos]); L is then the longest sequence
+    // EPI_QKVGQA*: GEMM columns [0, d) = q, [d, d + d_kv) = k, [d + d_kv, d + 2 d_kv) = v with d_kv = 128 n_kv_heads; k is
+    // [rows, d_kv], vt [B, n_kv_heads, 128, Lpad]. bias (nullable): bf16 [d + 2 d_kv], added before the first bf16 rounding
+    int n_kv_heads = 0;
+    const __nv_bfloat16* bias = nullptr;
 };
 
 // device map of a packed batch: seg_pos[r] = (sequence, position) of packed row r, for the rows of `segs`
@@ -154,13 +164,15 @@ void set_gemm_pair_mode(int on);
 int gemm_splitk_mode();
 void set_gemm_splitk_mode(int mode);
 
-// Lq > 0: q / out hold Lq query rows per batch row (a compact subset), k / vt the full L keys (token-cache forward)
+// Lq > 0: q / out hold Lq query rows per batch row (a compact subset), k / vt the full L keys (token-cache forward).
+// Hkv > 0 (grouped-query attention, H % Hkv == 0): k [B * L, 128 Hkv], vt [B, Hkv, 128, Lpad]; query head h reads kv head
+// h / (H / Hkv). 0 = H.
 int attention_fwd(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* vt, __nv_bfloat16* out, int B,
-                  int H, int L, int Lpad, float scale, cudaStream_t stream, int Lq = 0);
-// packed variable-length batch: q / k / out [segs.start[n], H * 128], vt [segs.n, H, 128, Lpad]; columns [L_s, Lpad) of
-// sequence s's V^T block must be finite zeros
+                  int H, int L, int Lpad, float scale, cudaStream_t stream, int Lq = 0, int Hkv = 0);
+// packed variable-length batch: q / out [segs.start[n], H * 128], k [segs.start[n], Hkv * 128], vt [segs.n, Hkv, 128, Lpad];
+// columns [L_s, Lpad) of sequence s's V^T block must be finite zeros
 int attention_packed_fwd(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* vt, __nv_bfloat16* out,
-                         const SegTable& segs, int H, int Lpad, float scale, cudaStream_t stream);
+                         const SegTable& segs, int H, int Lpad, float scale, cudaStream_t stream, int Hkv = 0);
 
 // err (nullable): device int, bit 0 is raised when an id is outside [0, vocab) (the kernel then reads row 0)
 int embed_rows(const int64_t* ids, const __nv_bfloat16* wte, __nv_bfloat16* x, int M, int d, int64_t vocab,

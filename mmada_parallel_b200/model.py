@@ -39,16 +39,38 @@ def rope_tables(head_dim: int, theta: float, seq_len: int) -> Tuple[torch.Tensor
 _PRECISIONS = {"bf16": _lib.PRECISION_BF16, "fp8": _lib.PRECISION_FP8}
 
 _BLOCK_KEYS = ("q_proj", "k_proj", "v_proj", "attn_out", "ff_proj", "up_proj", "ff_out", "attn_norm", "ff_norm")
+_QKV_BIAS_KEYS = ("q_proj", "k_proj", "v_proj")  # their `.bias` with config.include_qkv_bias -> blocks.<i>.q_bias|k_bias|v_bias
 
 
-def check_supported_config(config, n_heads: int) -> None:
+def effective_n_kv_heads(config, n_heads: int) -> int:
+    """ModelConfig.effective_n_kv_heads of the reference (configuration_llada.py:366-384): n_kv_heads, or 1 with
+    multi_query_attention=True, or n_heads; setting both inconsistently is an error. The result must divide n_heads."""
+    n_kv, mqa = getattr(config, "n_kv_heads", None), getattr(config, "multi_query_attention", None)
+    if n_kv is None:
+        h = 1 if mqa is True else n_heads
+    elif mqa is None:
+        h = int(n_kv)
+    else:
+        h = 1 if mqa else n_heads
+        if int(n_kv) != h:
+            raise ValueError("You can't set `multi_query_attention` and `n_kv_heads` at the same time.")
+    if h < 1 or n_heads % h:
+        raise ValueError(f"n_kv_heads={h} must divide n_heads={n_heads}")
+    return h
+
+
+def check_supported_config(config, n_heads: int, grouped_query: bool = False) -> int:
     """Features of the reference config this path does not implement must fail loudly, not silently differ (shared by the
-    single-GPU and the tensor-parallel model)."""
+    single-GPU and the tensor-parallel model). Returns the number of kv heads. grouped_query: the caller runs
+    n_kv_heads < n_heads and include_qkv_bias (the single-GPU model); the tensor-parallel model, which can only be
+    checked on several GPUs, refuses both."""
     g = lambda k, dflt=None: getattr(config, k, dflt)
-    if g("n_kv_heads") not in (None, n_heads):
-        raise NotImplementedError("GQA/MQA (n_kv_heads != n_heads) is not on the MMaDA-Parallel hot path")
-    for flag in ("alibi", "include_bias", "include_qkv_bias", "weight_tying", "scale_logits", "input_emb_norm",
-                 "attention_layer_norm"):
+    n_kv = effective_n_kv_heads(config, n_heads)
+    if not grouped_query and n_kv != n_heads:
+        raise NotImplementedError("GQA/MQA (n_kv_heads != n_heads) is not implemented by the tensor-parallel model")
+    if not grouped_query and g("include_qkv_bias", False):
+        raise NotImplementedError("config.include_qkv_bias=True is not implemented by the tensor-parallel model")
+    for flag in ("alibi", "include_bias", "weight_tying", "scale_logits", "input_emb_norm", "attention_layer_norm"):
         if g(flag, False):
             raise NotImplementedError(f"config.{flag}=True is not supported by the H100 hot path")
     if not g("rope", True) or not g("rope_full_precision", True):
@@ -60,6 +82,7 @@ def check_supported_config(config, n_heads: int) -> None:
         v = getattr(v, "value", v)  # the reference uses StrEnum members
         if v is not None and str(v).lower() not in ok:
             raise NotImplementedError(f"config.{key}={v!r} is not supported by the H100 hot path (needs one of {ok})")
+    return n_kv
 
 
 class LLaDAForMultiModalGeneration:
@@ -88,11 +111,13 @@ class LLaDAForMultiModalGeneration:
         self.max_seq_len = int(max_seq_len or g("max_sequence_length", 4096))
         self.max_batch = int(max_batch)
         self.precision = precision
-        check_supported_config(config, self.n_heads)
+        self.n_kv_heads = check_supported_config(config, self.n_heads, grouped_query=True)
+        self.qkv_bias = bool(g("include_qkv_bias", False))
         cfg = _lib.ModelConfig(self.d_model, self.n_heads, self.n_layers, self.mlp_hidden, self.vocab_rows,
                                self.max_seq_len, self.max_batch, self.rms_eps)
         handle = C.c_void_p()
-        check(lib.mmdp_model_create_ex(C.byref(cfg), _PRECISIONS[precision], C.byref(handle)))
+        check(lib.mmdp_model_create_arch(C.byref(cfg), _PRECISIONS[precision], self.n_kv_heads,
+                                         _lib.ARCH_QKV_BIAS if self.qkv_bias else 0, C.byref(handle)))
         self._h = handle
         cos, sin = rope_tables(self.d_model // self.n_heads, self.rope_theta, self.max_seq_len)
         check(lib.mmdp_model_set_rope(self._h, cos.data_ptr(), sin.data_ptr(), self.max_seq_len, stream_ptr()))
@@ -109,7 +134,9 @@ class LLaDAForMultiModalGeneration:
     # weights
     # ------------------------------------------------------------------------------------------------------------
     @staticmethod
-    def _native_name(hf_name: str) -> Optional[str]:
+    def _native_name(hf_name: str, qkv_bias: bool = False) -> Optional[str]:
+        """Native tensor name of a state-dict key (None: not a weight of the native context). qkv_bias: the context holds the
+        q/k/v_proj biases (config.include_qkv_bias)."""
         n = hf_name
         if n.startswith("model."):
             n = n[len("model."):]
@@ -125,10 +152,12 @@ class LLaDAForMultiModalGeneration:
             parts = n.split(".")
             if len(parts) == 4 and parts[3] == "weight" and parts[2] in _BLOCK_KEYS:
                 return f"blocks.{parts[1]}.{parts[2]}"
+            if len(parts) == 4 and parts[3] == "bias" and parts[2] in _QKV_BIAS_KEYS and qkv_bias:
+                return f"blocks.{parts[1]}.{parts[2][0]}_bias"
         return None
 
     def set_weight(self, hf_name: str, tensor: torch.Tensor) -> bool:
-        name = self._native_name(hf_name)
+        name = self._native_name(hf_name, self.qkv_bias)
         if name is None:
             return False
         t = tensor.detach().to(torch.bfloat16).contiguous()
@@ -143,7 +172,8 @@ class LLaDAForMultiModalGeneration:
         items = state_dict.items() if hasattr(state_dict, "items") else state_dict
         unexpected = [k for k, v in items if not self.set_weight(k, v)]
         torch.cuda.synchronize()
-        expected = {"wte", "ln_f", "head"} | {f"blocks.{i}.{k}" for i in range(self.n_layers) for k in _BLOCK_KEYS}
+        keys = _BLOCK_KEYS + (("q_bias", "k_bias", "v_bias") if self.qkv_bias else ())
+        expected = {"wte", "ln_f", "head"} | {f"blocks.{i}.{k}" for i in range(self.n_layers) for k in keys}
         missing = sorted(expected - self._loaded)
         if strict and (missing or unexpected):
             raise KeyError(f"load_state_dict: missing={missing[:8]} unexpected={unexpected[:8]}")
@@ -204,6 +234,9 @@ class LLaDAForMultiModalGeneration:
         `to_compute_mask [B, L]` embeds only the masked tokens, refreshes their keys / values inside the caches, attends from them
         to ALL cached keys, and scatters their logits into the logit cache. Returns the logit cache itself, like the reference
         (the tensor is updated in place by later calls)."""
+        if self.n_kv_heads != self.n_heads or self.qkv_bias:
+            raise NotImplementedError("the token-cache forward needs n_kv_heads == n_heads without a q/k/v bias: the reference's "
+                                      "cache is zeros_like(x) (modeling_llada.py:930-932) and cannot hold d_kv-wide keys")
         B, L = ids.shape
         Lpad = (L + 7) // 8 * 8
         ent = self._cache.get(cat)
