@@ -196,6 +196,13 @@ MMDP_API int mmdp_attention(const uint16_t* q, const uint16_t* k, const uint16_t
  * attends to its own keys only; its pad columns vt[i, ..., seg_len[i]:Lpad] must hold finite values (they meet P == 0). */
 MMDP_API int mmdp_attention_packed(const uint16_t* q, const uint16_t* k, const uint16_t* vt, uint16_t* out, int n_seg, const int32_t* seg_len,
                                    int n_heads, int Lpad, float scale, void* stream);
+/* The packed batch with a query ROW WINDOW per sequence: sequence i computes its query rows [win_lo[i], win_hi[i]) only (host int32,
+ * 0 <= lo < hi <= seg_len[i]), each against all of its keys. out holds the windows end to end: [sum (hi - lo), n_heads*128], window
+ * i starting at row sum_{j<i} (win_hi[j] - win_lo[j]). k: [sum seg_len, n_kv_heads*128]; vt: [n_seg, n_kv_heads, 128, Lpad];
+ * n_kv_heads == n_heads runs the multi-head kernels, a divisor of n_heads the grouped-query ones. */
+MMDP_API int mmdp_attention_packed_window(const uint16_t* q, const uint16_t* k, const uint16_t* vt, uint16_t* out, int n_seg,
+                                          const int32_t* seg_len, const int32_t* win_lo, const int32_t* win_hi, int n_heads,
+                                          int n_kv_heads, int Lpad, float scale, void* stream);
 /* Grouped-query attention (modeling_llada.py:660-679: k / v repeat_interleave'd to n_heads): n_kv_heads divides n_heads and query
  * head h attends with kv head h / (n_heads / n_kv_heads). k: [rows, n_kv_heads*128]; vt: [B or n_seg, n_kv_heads, 128, Lpad];
  * q / out as above. seg_len == NULL: B sequences of L rows each (mmdp_attention); otherwise the packed batch of n_seg = B
@@ -408,6 +415,16 @@ MMDP_API int mmdp_model_forward_window(mmdp_model* m, const int64_t* ids, int B,
 MMDP_API int mmdp_model_forward_packed(mmdp_model* m, const int64_t* ids, int n_seg, const int32_t* seg_len, const int32_t* rows_a,
                                        int n_a, uint16_t* out_a, const int32_t* rows_b, int n_b, int col0_b, int ncols_b, uint16_t* out_b,
                                        void* stream);
+/* mmdp_model_forward_packed with a last-block ROW WINDOW per sequence: win_lo / win_hi (host int32, both NULL for none) give
+ * sequence i's window [win_lo[i], win_hi[i]), 0 <= lo < hi <= seg_len[i]. Every row of rows_a / rows_b must be a position inside
+ * its sequence's window; the last block computes its attention output and MLP for the window rows only (keys and values of all
+ * rows are still computed), on a compact copy of them. A row outside its window raises bit 2 of the error flags and a row
+ * outside the packed batch bit 1; neither is read. The head outputs are those of mmdp_model_forward_packed (identical GEMM rows;
+ * attention rows differ only by which query tiles take the KV-split path). MMDP_ROW_WINDOW=0 ignores the windows. After a
+ * windowed forward mmdp_model_hidden holds the input of the last block. */
+MMDP_API int mmdp_model_forward_packed_window(mmdp_model* m, const int64_t* ids, int n_seg, const int32_t* seg_len, const int32_t* win_lo,
+                                              const int32_t* win_hi, const int32_t* rows_a, int n_a, uint16_t* out_a, const int32_t* rows_b,
+                                              int n_b, int col0_b, int ncols_b, uint16_t* out_b, void* stream);
 
 /* Debug/testing: copy of the residual stream after `layer` layers is kept when enabled (device pointer returned). */
 MMDP_API const uint16_t* mmdp_model_hidden(mmdp_model* m);
@@ -422,7 +439,8 @@ MMDP_API int mmdp_model_forward_cached(mmdp_model* m, const int64_t* ids, int B,
                               uint16_t* vtcache, uint16_t* logits, void* stream);
 /* Sticky device-side error flags of the forwards issued so far, read and cleared (this call SYNCHRONISES `stream`):
  * bit 0 = a token id was outside [0, vocab_size) (torch raises IndexError in nn.Embedding; the kernel read row 0),
- * bit 1 = a logits row index (rows_a / rows_b) was outside [0, B*L). The host mirrors call it at their read-back point. */
+ * bit 1 = a logits row index (rows_a / rows_b) was outside [0, B*L), bit 2 = one was outside the last block's row window
+ * (mmdp_model_forward_window, mmdp_model_forward_packed_window). The host mirrors call it at their read-back point. */
 MMDP_API int mmdp_model_error_flags(mmdp_model* m, int32_t* flags_host, void* stream);
 
 #ifdef __cplusplus

@@ -108,6 +108,7 @@ SIGNATURES = {
     "mmdp_resid_add_f32": (_i, [_vp, _i, _vp, _i, _i, _i, _vp]),
     "mmdp_attention": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp]),
     "mmdp_attention_packed": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _f, _vp]),
+    "mmdp_attention_packed_window": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _f, _vp]),
     "mmdp_attention_gqa": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _f, _vp]),
     "mmdp_rmsnorm": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _f, _vp]),
     "mmdp_embed": (_i, [_vp, _vp, _vp, _i, _i, _i64, _vp]),
@@ -141,6 +142,7 @@ SIGNATURES = {
     "mmdp_model_forward": (_i, [_vp, _vp, _i, _i, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp, _vp]),
     "mmdp_model_forward_window": (_i, [_vp, _vp, _i, _i, _vp, _i, _vp, _vp, _i, _i, _i, _vp, _i, _i, _vp]),
     "mmdp_model_forward_packed": (_i, [_vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp, _vp]),
+    "mmdp_model_forward_packed_window": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp, _vp]),
     "mmdp_model_forward_cached": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "mmdp_model_hidden": (_vp, [_vp]),
     "mmdp_model_error_flags": (_i, [_vp, C.POINTER(C.c_int32), _vp]),
@@ -260,6 +262,22 @@ def attention_packed(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, seq_len
     out = torch.empty_like(q)
     check(lib.mmdp_attention_packed(ptr(q), ptr(k), ptr(vt), ptr(out), len(seq_lens), lens, n_heads, vt.shape[-1], scale,
                                     stream_ptr()))
+    return out
+
+
+def attention_packed_window(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, seq_lens, windows, n_heads: int, scale: float,
+                            n_kv_heads: int = 0) -> torch.Tensor:
+    """Packed attention for the query rows [lo, hi) of every sequence only: windows = [(lo, hi)] per sequence. q [sum(seq_lens),
+    n_heads * 128], k [sum(seq_lens), n_kv_heads * 128] and vt [len(seq_lens), n_kv_heads, 128, Lpad] as in attention_packed
+    (n_kv_heads 0: n_heads). Returns the windows' rows end to end, [sum(hi - lo), n_heads * 128]."""
+    require_cuda(q, k, vt)
+    n = len(seq_lens)
+    lens = (C.c_int32 * n)(*[int(x) for x in seq_lens])
+    lo = (C.c_int32 * n)(*[int(w[0]) for w in windows])
+    hi = (C.c_int32 * n)(*[int(w[1]) for w in windows])
+    out = torch.empty((sum(int(w[1]) - int(w[0]) for w in windows), q.shape[1]), dtype=q.dtype, device=q.device)
+    check(lib.mmdp_attention_packed_window(ptr(q), ptr(k), ptr(vt), ptr(out), n, lens, lo, hi, n_heads, n_kv_heads or n_heads,
+                                           vt.shape[-1], scale, stream_ptr()))
     return out
 
 

@@ -3,6 +3,7 @@
 // block :906-972). No torch types cross this boundary.
 #include "../../include/mmdp.h"
 #include "mmdp_internal.h"
+#include "ptx.cuh"
 
 #include <stdlib.h>
 #include <string.h>
@@ -37,6 +38,67 @@ int packed_row_map(const SegTable& segs, int2* seg_pos, cudaStream_t stream) {
     const int M = segs.start[segs.n];
     LaunchScope ls(LK_ROW, 8.0 * M, stream);
     packed_row_map_kernel<<<(M + 255) / 256, 256, 0, stream>>>(segs, seg_pos);
+    MMDP_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// Last-block row windows of a packed forward: sequence s (packed rows [start[s], start[s + 1])) keeps its positions [lo[s], hi[s]),
+// stored as compact rows [out0[s], out0[s + 1]), the windows of all sequences end to end.
+struct WinTable {
+    int n;
+    int start[kMaxSegs + 1];
+    int lo[kMaxSegs], hi[kMaxSegs];
+    int out0[kMaxSegs + 1];
+};
+
+// xc[j] = x[packed row of compact row j], one CTA per compact row, 16-byte moves
+__global__ void __launch_bounds__(128) window_gather_kernel(const __grid_constant__ WinTable w, const bf16* __restrict__ x,
+                                                            bf16* __restrict__ xc, int d) {
+    const int j = blockIdx.x;
+    pdl_launch_dependents();
+    pdl_wait();
+    int s = 0;
+    for (int i = 1; i < w.n; ++i)
+        if (j >= w.out0[i]) s = i;
+    const int r = w.start[s] + w.lo[s] + (j - w.out0[s]);
+    const uint4* src = reinterpret_cast<const uint4*>(x + (size_t)r * d);
+    uint4* dst = reinterpret_cast<uint4*>(xc + (size_t)j * d);
+    for (int i = threadIdx.x; i < d / 8; i += blockDim.x) dst[i] = src[i];
+}
+
+int window_gather(const WinTable& w, const bf16* x, bf16* xc, int d, cudaStream_t stream) {
+    const int Mw = w.out0[w.n];
+    LaunchScope ls(LK_ROW, 2.0 * Mw * (double)d * 2, stream);
+    MMDP_CUDA(launch_ex(window_gather_kernel, dim3(Mw), dim3(128), 0, stream, pdl_mode() != 0, false, w, x, xc, d));
+    return 0;
+}
+
+// Packed row -> compact row of the head's requested rows: out[i] = the compact row of packed row rows[i]. A row outside the
+// packed batch raises bit 1 of *err, a row outside its sequence's window bit 2 (the "row outside the window" flag of
+// mmdp_model_forward_window); both then read compact row 0.
+__global__ void window_row_map_kernel(const __grid_constant__ WinTable w, const int32_t* __restrict__ rows, int n,
+                                      int32_t* __restrict__ out, int* __restrict__ err) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int r = rows[i];
+    int c = 0;
+    if (r < 0 || r >= w.start[w.n]) {
+        atomicOr(err, 2);
+    } else {
+        int s = 0;
+        for (int k = 1; k < w.n; ++k)
+            if (r >= w.start[k]) s = k;
+        const int p = r - w.start[s];
+        if (p < w.lo[s] || p >= w.hi[s]) atomicOr(err, 4);
+        else c = w.out0[s] + p - w.lo[s];
+    }
+    out[i] = c;
+}
+
+int window_row_map(const WinTable& w, const int32_t* rows, int n, int32_t* out, int* err, cudaStream_t stream) {
+    if (n <= 0) return 0;
+    LaunchScope ls(LK_ROW, 8.0 * n, stream);
+    window_row_map_kernel<<<(n + 255) / 256, 256, 0, stream>>>(w, rows, n, out, err);
     MMDP_CUDA(cudaGetLastError());
     return 0;
 }
@@ -84,12 +146,13 @@ struct mmdp_model {
     // workspace
     int Mmax = 0, Lpad_max = 0;
     bf16 *x = nullptr, *xn = nullptr, *q = nullptr, *k = nullptr, *vt = nullptr, *att = nullptr, *h = nullptr, *xr = nullptr;
-    int* err_flag = nullptr;  // device: bit 0 = token id out of range, bit 1 = logits row index out of range
+    int* err_flag = nullptr;  // device: bit 0 = token id out of range, bit 1 = logits row index out of range, bit 2 = row outside the window
     // V^T pad rule (vt_prepare): vt_Lpad = column stride of the layout the buffer was last zeroed for, vt_len[s] = columns
     // of block s written since then
     int vt_Lpad = 0;
     std::vector<int> vt_len;
     int2* seg_pos = nullptr;  // packed forward: (sequence, position) of every packed row
+    int32_t* win_rows = nullptr;  // packed forward with row windows: the compact rows of the head's requested rows
     int precision = MMDP_PRECISION_BF16;
     uint8_t* a8 = nullptr;  // FP8: the quantised input of the current linear, [M, K] e4m3
     float* as = nullptr;    // FP8: its scales, [K / 128][M]
@@ -169,6 +232,18 @@ MMDP_API int mmdp_attention_packed(const uint16_t* q, const uint16_t* k, const u
     segs.n = n_seg;
     for (int i = 0; i < n_seg; ++i) segs.start[i + 1] = segs.start[i] + seg_len[i];
     return attention_packed_fwd((const bf16*)q, (const bf16*)k, (const bf16*)vt, (bf16*)out, segs, n_heads, Lpad, scale, (cudaStream_t)stream);
+}
+
+MMDP_API int mmdp_attention_packed_window(const uint16_t* q, const uint16_t* k, const uint16_t* vt, uint16_t* out, int n_seg,
+                                          const int32_t* seg_len, const int32_t* win_lo, const int32_t* win_hi, int n_heads,
+                                          int n_kv_heads, int Lpad, float scale, void* stream) {
+    if (!seg_len || !win_lo || !win_hi || n_seg <= 0 || n_seg > kMaxSegs)
+        return set_error("mmdp_attention_packed_window: %d sequences (1 to %d) with lengths and windows", n_seg, kMaxSegs);
+    SegTable segs{};
+    segs.n = n_seg;
+    for (int i = 0; i < n_seg; ++i) segs.start[i + 1] = segs.start[i] + seg_len[i];
+    return attention_packed_fwd((const bf16*)q, (const bf16*)k, (const bf16*)vt, (bf16*)out, segs, n_heads, Lpad, scale, (cudaStream_t)stream,
+                                n_kv_heads, win_lo, win_hi);
 }
 
 MMDP_API int mmdp_attention_gqa(const uint16_t* q, const uint16_t* k, const uint16_t* vt, uint16_t* out, int B, const int32_t* seg_len,
@@ -479,6 +554,7 @@ MMDP_API int mmdp_model_create_arch(const mmdp_model_config* c, int precision, i
     rc |= dev_alloc(m, (void**)&m->sin_tab, (size_t)c->max_seq_len * 64 * 4);
     rc |= dev_alloc(m, (void**)&m->err_flag, sizeof(int));
     rc |= dev_alloc(m, (void**)&m->seg_pos, Mm * sizeof(int2));
+    rc |= dev_alloc(m, (void**)&m->win_rows, Mm * sizeof(int32_t));
     m->vt_len.assign(c->max_batch, 0);
     if (!rc && cudaMemset(m->err_flag, 0, sizeof(int)) != cudaSuccess) rc = set_error("mmdp_model_create: cudaMemset failed");
     if (rc) {
@@ -646,22 +722,26 @@ static int vt_prepare(mmdp_model* m, int n, const int* lens, int Lpad, cudaStrea
 }
 
 // ln_f + LM head on the gathered rows (rows_a: all V columns; rows_b: columns [col0_b, col0_b + ncols_b)) of the M rows in
-// m->x. row_lo / row_hi / L: the last block's row window (0: none); a row outside it raises bit 2 of the error flag.
+// x (m->x when null), normalised into xr (m->xr when null). row_lo / row_hi / L: the last block's row window (0: none); a row
+// outside it raises bit 2 of the error flag.
 static int head_rows(mmdp_model* m, int M, const int32_t* rows_a, int n_a, uint16_t* out_a, const int32_t* rows_b, int n_b,
-                     int col0_b, int ncols_b, uint16_t* out_b, int row_lo, int row_hi, int L, cudaStream_t s) {
+                     int col0_b, int ncols_b, uint16_t* out_b, int row_lo, int row_hi, int L, cudaStream_t s,
+                     const bf16* x = nullptr, bf16* xr = nullptr) {
     const mmdp_model_config& c = m->cfg;
     const int d = c.d_model, V = c.vocab_size;
+    if (!x) x = m->x;
+    if (!xr) xr = m->xr;
     if (n_a > 0) {
         if (!rows_a || !out_a) return set_error("mmdp_model_forward: rows_a/out_a null");
         if (n_a > m->Mmax) return set_error("mmdp_model_forward: too many rows_a");
-        if (rmsnorm_rows(m->x, d, rows_a, m->ln_f, m->xr, d, n_a, d, c.rms_eps, s, M, m->err_flag, row_lo, row_hi, L)) return -1;
-        if (gemm_bf16(EPI_PLAIN, m->xr, d, m->head, d, n_a, V, d, (bf16*)out_a, V, nullptr, 0, nullptr, s)) return -1;
+        if (rmsnorm_rows(x, d, rows_a, m->ln_f, xr, d, n_a, d, c.rms_eps, s, M, m->err_flag, row_lo, row_hi, L)) return -1;
+        if (gemm_bf16(EPI_PLAIN, xr, d, m->head, d, n_a, V, d, (bf16*)out_a, V, nullptr, 0, nullptr, s)) return -1;
     }
     if (n_b > 0) {
         if (!rows_b || !out_b) return set_error("mmdp_model_forward: rows_b/out_b null");
         if (n_a + n_b > m->Mmax) return set_error("mmdp_model_forward: too many rows_a + rows_b");
-        bf16* xr_b = m->xr + (size_t)n_a * d;
-        if (rmsnorm_rows(m->x, d, rows_b, m->ln_f, xr_b, d, n_b, d, c.rms_eps, s, M, m->err_flag, row_lo, row_hi, L)) return -1;
+        bf16* xr_b = xr + (size_t)n_a * d;
+        if (rmsnorm_rows(x, d, rows_b, m->ln_f, xr_b, d, n_b, d, c.rms_eps, s, M, m->err_flag, row_lo, row_hi, L)) return -1;
         if (gemm_bf16(EPI_PLAIN, xr_b, d, m->head + (size_t)col0_b * d, d, n_b, ncols_b, d, (bf16*)out_b, ncols_b, nullptr, 0, nullptr, s)) return -1;
     }
     return 0;
@@ -749,28 +829,50 @@ MMDP_API int mmdp_model_forward_window(mmdp_model* m, const int64_t* ids, int B,
     return model_forward(m, ids, B, L, nullptr, rows_a, n_a, out_a, rows_b, n_b, col0_b, ncols_b, out_b, row_lo, row_hi, stream);
 }
 
-MMDP_API int mmdp_model_forward_packed(mmdp_model* m, const int64_t* ids, int n_seg, const int32_t* seg_len, const int32_t* rows_a,
-                                       int n_a, uint16_t* out_a, const int32_t* rows_b, int n_b, int col0_b, int ncols_b, uint16_t* out_b,
-                                       void* stream) {
+// Packed forward; win_lo / win_hi (host, both null or both set): the last block's row window [win_lo[s], win_hi[s]) of every
+// sequence s. Layers 0 .. n-2 and the last block's norm + QKV run on all M packed rows (keys and values of every row). With
+// windows, the window rows of x are then gathered into m->xr, and the rest of the last block (attention, attn_out + residual,
+// ff_norm, SwiGLU, ff_out + residual) runs on those Mw compact rows; the head reads them through the row map (ln_f into m->xn).
+// m->x then keeps the input of the last block.
+static int forward_packed(mmdp_model* m, const int64_t* ids, int n_seg, const int32_t* seg_len, const int32_t* win_lo,
+                          const int32_t* win_hi, const int32_t* rows_a, int n_a, uint16_t* out_a, const int32_t* rows_b, int n_b,
+                          int col0_b, int ncols_b, uint16_t* out_b, void* stream) {
     if (!m || !ids || !seg_len) return set_error("mmdp_model_forward_packed: null argument");
     const mmdp_model_config& c = m->cfg;
     if (n_seg <= 0 || n_seg > c.max_batch || n_seg > kMaxSegs)
         return set_error("mmdp_model_forward_packed: %d sequences outside [1, %d] (max_batch, at most %d)", n_seg, c.max_batch, kMaxSegs);
+    if (!win_lo != !win_hi) return set_error("mmdp_model_forward_packed_window: give both win_lo and win_hi, or neither");
     SegTable segs{};
     segs.n = n_seg;
     int Lmax = 0;
     for (int i = 0; i < n_seg; ++i) {
         if (seg_len[i] <= 0 || seg_len[i] > c.max_seq_len)
             return set_error("mmdp_model_forward_packed: sequence %d has length %d (max_seq_len=%d)", i, seg_len[i], c.max_seq_len);
+        if (win_lo && (win_lo[i] < 0 || win_lo[i] >= win_hi[i] || win_hi[i] > seg_len[i]))
+            return set_error("mmdp_model_forward_packed_window: sequence %d of length %d has the window [%d, %d)", i, seg_len[i],
+                             win_lo[i], win_hi[i]);
         segs.start[i + 1] = segs.start[i] + seg_len[i];
         Lmax = seg_len[i] > Lmax ? seg_len[i] : Lmax;
     }
     if (Lmax > m->rope_len) return set_error("mmdp_model_forward_packed: rotary table covers %d positions, need %d", m->rope_len, Lmax);
     if (n_b > 0 && (col0_b < 0 || ncols_b <= 0 || col0_b + ncols_b > c.vocab_size || (ncols_b % 8)))
         return set_error("mmdp_model_forward_packed: bad column window [%d,+%d)", col0_b, ncols_b);
+    // windows that cover whole sequences skip nothing; MMDP_ROW_WINDOW=0 switches them off (A/B switch)
+    WinTable wt{};
+    bool window = false;
+    if (win_lo && opt(OPT_ROW_WINDOW)) {
+        wt.n = n_seg;
+        for (int i = 0; i < n_seg; ++i) {
+            wt.start[i + 1] = segs.start[i + 1];
+            wt.lo[i] = win_lo[i];
+            wt.hi[i] = win_hi[i];
+            wt.out0[i + 1] = wt.out0[i] + win_hi[i] - win_lo[i];
+            window = window || win_hi[i] - win_lo[i] < seg_len[i];
+        }
+    }
     cudaStream_t s = (cudaStream_t)stream;
     const int d = c.d_model, ff = c.mlp_hidden, V = c.vocab_size, H = c.n_heads, Hkv = m->n_kv_heads;
-    const int M = segs.start[n_seg];
+    const int M = segs.start[n_seg], Mw = window ? wt.out0[n_seg] : M;
     const int Lpad = ((Lmax + 7) / 8) * 8;
     if (vt_prepare(m, n_seg, seg_len, Lpad, s)) return -1;
     if (packed_row_map(segs, m->seg_pos, s)) return -1;
@@ -782,16 +884,41 @@ MMDP_API int mmdp_model_forward_packed(mmdp_model* m, const int64_t* ids, int n_
     const int qkv_epi = m->gqa() ? EPI_QKVGQA_PACKED : EPI_QKVROPE_PACKED;
     for (int li = 0; li < c.n_layers; ++li) {
         const LayerWeights& l = m->layers[li];
+        const bool win = window && li == c.n_layers - 1;
+        bf16* x = win ? m->xr : m->x;  // the residual stream of the rows this block finishes, Mb of them
+        const int Mb = win ? Mw : M;
         qa.bias = l.qkv_bias;
         if (rmsnorm(m->x, d, l.attn_norm, m->xn, d, M, d, c.rms_eps, s)) return -1;
         if (block_linear(m, l, LIN_QKV, qkv_epi, m->xn, d, M, nullptr, 0, nullptr, 0, &qa, s)) return -1;
-        if (attention_packed_fwd(m->q, m->k, m->vt, m->att, segs, H, Lpad, scale, s, Hkv)) return -1;
-        if (block_linear(m, l, LIN_O, EPI_RESID, m->att, d, M, m->x, d, m->x, d, nullptr, s)) return -1;
-        if (rmsnorm(m->x, d, l.ff_norm, m->xn, d, M, d, c.rms_eps, s)) return -1;
-        if (block_linear(m, l, LIN_13, EPI_SWIGLU, m->xn, d, M, m->h, ff, nullptr, 0, nullptr, s)) return -1;
-        if (block_linear(m, l, LIN_2, EPI_RESID, m->h, ff, M, m->x, d, m->x, d, nullptr, s)) return -1;
+        if (win) {
+            if (window_gather(wt, m->x, m->xr, d, s)) return -1;
+            if (attention_packed_fwd(m->q, m->k, m->vt, m->att, segs, H, Lpad, scale, s, Hkv, wt.lo, wt.hi)) return -1;
+        } else {
+            if (attention_packed_fwd(m->q, m->k, m->vt, m->att, segs, H, Lpad, scale, s, Hkv)) return -1;
+        }
+        if (block_linear(m, l, LIN_O, EPI_RESID, m->att, d, Mb, x, d, x, d, nullptr, s)) return -1;
+        if (rmsnorm(x, d, l.ff_norm, m->xn, d, Mb, d, c.rms_eps, s)) return -1;
+        if (block_linear(m, l, LIN_13, EPI_SWIGLU, m->xn, d, Mb, m->h, ff, nullptr, 0, nullptr, s)) return -1;
+        if (block_linear(m, l, LIN_2, EPI_RESID, m->h, ff, Mb, x, d, x, d, nullptr, s)) return -1;
     }
-    return head_rows(m, M, rows_a, n_a, out_a, rows_b, n_b, col0_b, ncols_b, out_b, 0, 0, 0, s);
+    if (!window) return head_rows(m, M, rows_a, n_a, out_a, rows_b, n_b, col0_b, ncols_b, out_b, 0, 0, 0, s);
+    if (n_a + n_b > m->Mmax) return set_error("mmdp_model_forward_packed_window: too many rows_a + rows_b");
+    if ((n_a > 0 && !rows_a) || (n_b > 0 && !rows_b)) return set_error("mmdp_model_forward_packed_window: rows_a/rows_b null");
+    if (window_row_map(wt, rows_a, n_a, m->win_rows, m->err_flag, s)) return -1;
+    if (window_row_map(wt, rows_b, n_b, m->win_rows + n_a, m->err_flag, s)) return -1;
+    return head_rows(m, Mw, m->win_rows, n_a, out_a, m->win_rows + n_a, n_b, col0_b, ncols_b, out_b, 0, 0, 0, s, m->xr, m->xn);
+}
+
+MMDP_API int mmdp_model_forward_packed(mmdp_model* m, const int64_t* ids, int n_seg, const int32_t* seg_len, const int32_t* rows_a,
+                                       int n_a, uint16_t* out_a, const int32_t* rows_b, int n_b, int col0_b, int ncols_b, uint16_t* out_b,
+                                       void* stream) {
+    return forward_packed(m, ids, n_seg, seg_len, nullptr, nullptr, rows_a, n_a, out_a, rows_b, n_b, col0_b, ncols_b, out_b, stream);
+}
+
+MMDP_API int mmdp_model_forward_packed_window(mmdp_model* m, const int64_t* ids, int n_seg, const int32_t* seg_len, const int32_t* win_lo,
+                                              const int32_t* win_hi, const int32_t* rows_a, int n_a, uint16_t* out_a, const int32_t* rows_b,
+                                              int n_b, int col0_b, int ncols_b, uint16_t* out_b, void* stream) {
+    return forward_packed(m, ids, n_seg, seg_len, win_lo, win_hi, rows_a, n_a, out_a, rows_b, n_b, col0_b, ncols_b, out_b, stream);
 }
 
 MMDP_API int mmdp_model_forward_cached(mmdp_model* m, const int64_t* ids, int B, int L, int Tq, const int32_t* pos_map, uint16_t* kcache,

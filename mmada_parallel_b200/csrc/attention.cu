@@ -9,7 +9,9 @@
 //   * attention_packed_kernel runs the same body over a packed variable-length batch: work items enumerate
 //     (sequence, head, query tile), each sequence attends to its own keys only (attention_packed_fwd);
 //   * grouped-query attention (kGqa): query head h reads kv head h / kv_group of k [rows, 128 Hkv] and V^T [B][Hkv][128][Lpad];
-//     separate kernels, so that the multi-head ones keep their code.
+//     separate kernels, so that the multi-head ones keep their code;
+//   * attention_packed_window_kernel (kWin): a packed batch where sequence s queries only its rows [lo_s, hi_s) (against all of
+//     its keys) and writes them to a compact output, the windows of all sequences end to end (last-block row windows).
 #include "mmdp_internal.h"
 #include "ptx.cuh"
 
@@ -45,14 +47,22 @@ struct AttnSegs {
     int tile0[kMaxSegs + 1];
 };
 
+// Row windows of a packed launch: sequence s's queries are its rows [q0[s], q0[s] + nq[s]); their outputs are rows
+// [out0[s], out0[s] + nq[s]) of the compact output. segs.tile0 counts the windows' query tiles; keys stay whole sequences.
+struct AttnWin {
+    AttnSegs segs;
+    int q0[kMaxSegs], nq[kMaxSegs], out0[kMaxSegs];
+};
+
 // One CTA's work item. kPacked = false: B sequences of L keys / Lq queries each, laid out batch row after batch row (the
 // kernel parameters). kPacked = true: the sequences of `segs`, each with its own length (L = Lq = its length).
-// kGqa: H / kv_group kv heads, query head h reads kv head h / kv_group.
-template <int kBKV, bool kPacked, bool kGqa = false>
+// kGqa: H / kv_group kv heads, query head h reads kv head h / kv_group. kWin (with kPacked, segs = &win->segs): the row windows
+// of `win`.
+template <int kBKV, bool kPacked, bool kGqa = false, bool kWin = false>
 __device__ __forceinline__ void attention_body(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmVt,
                                                __nv_bfloat16* __restrict__ out, int H, int L, int d_model, float scale_log2,
                                                int n_full, int splits, float* __restrict__ part_ws, int Lq, const AttnSegs* segs,
-                                               int kv_group = 1) {
+                                               int kv_group = 1, const AttnWin* win = nullptr) {
     constexpr int kKBytes = AttnCfg<kBKV>::kKBytes, kVBytes = AttnCfg<kBKV>::kVBytes;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -80,13 +90,19 @@ __device__ __forceinline__ void attention_body(const CUtensorMap& tmQ, const CUt
         piece = t - (t / splits) * splits;
     }
     // packed: the tile's sequence (a uniform scan of the small table), its first row and length; keys past its end are masked
-    // through nvalid, query rows past it are not stored
-    int seg = 0, seg0 = 0, tl = tile;
+    // through nvalid, query rows past it are not stored. kWin: the first query row q0 and the first output row o0 of its window
+    int seg = 0, seg0 = 0, tl = tile, q0 = 0, o0 = 0;
     if constexpr (kPacked) {
         for (int i = 1; i < segs->n; ++i)
             if (tile >= segs->tile0[i]) seg = i;
         seg0 = segs->start[seg];
         L = Lq = segs->start[seg + 1] - seg0;
+        o0 = seg0;
+        if constexpr (kWin) {
+            q0 = win->q0[seg];
+            Lq = win->nq[seg];
+            o0 = win->out0[seg];
+        }
         n_qt = (Lq + 127) / 128;
         n_kv_all = (L + kBKV - 1) / kBKV;
         tl = tile - segs->tile0[seg];
@@ -122,7 +138,7 @@ __device__ __forceinline__ void attention_body(const CUtensorMap& tmQ, const CUt
         // ===================== TMA producer: Q, then K(j) and V^T(j) =====================
         setmaxnreg_dec<40>();
         if (warp == 0 && elect_one_sync()) {
-            const int qrow0 = (kPacked ? seg0 : b * Lq) + qt * 128;
+            const int qrow0 = (kPacked ? seg0 + q0 : b * Lq) + qt * 128;
             mbar_expect_tx(q_full, kQBytes);
             tma_load_2d(sQ, &tmQ, q_full, h * 128, qrow0);
             tma_load_2d(sQ + kQBytes / 2, &tmQ, q_full, h * 128 + 64, qrow0);
@@ -253,7 +269,7 @@ __device__ __forceinline__ void attention_body(const CUtensorMap& tmQ, const CUt
                 *reinterpret_cast<float2*>(slot + (size_t)r * 128 + 8 * jj + c0) = make_float2(o[4 * jj + 2 * hh], o[4 * jj + 2 * hh + 1]);
         } else {
             const float inv_l = 1.0f / l_run[hh];
-            __nv_bfloat16* orow = out + (size_t)((kPacked ? seg0 : b * Lq) + qrow) * d_model + h * 128;
+            __nv_bfloat16* orow = out + (size_t)((kPacked ? o0 : b * Lq) + qrow) * d_model + h * 128;
 #pragma unroll
             for (int jj = 0; jj < 16; ++jj)
                 *reinterpret_cast<uint32_t*>(orow + 8 * jj + c0) = pack_bf16x2(o[4 * jj + 2 * hh] * inv_l, o[4 * jj + 2 * hh + 1] * inv_l);
@@ -294,12 +310,23 @@ attention_packed_gqa_kernel(const __grid_constant__ CUtensorMap tmQ, const __gri
     attention_body<kBKV, true, true>(tmQ, tmK, tmVt, out, H, 0, d_model, scale_log2, n_full, splits, part_ws, 0, &segs, kv_group);
 }
 
+// multi-head (kGqa = false, kv_group unused) and grouped-query instantiations of the windowed packed launch
+template <int kBKV, bool kGqa>
+__global__ void __launch_bounds__(kAttnThreads, 1)
+attention_packed_window_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                               const __grid_constant__ CUtensorMap tmVt, __nv_bfloat16* __restrict__ out, int H, int d_model,
+                               float scale_log2, int n_full, int splits, float* __restrict__ part_ws, const __grid_constant__ AttnWin win,
+                               int kv_group) {
+    attention_body<kBKV, true, kGqa, true>(tmQ, tmK, tmVt, out, H, 0, d_model, scale_log2, n_full, splits, part_ws, 0, &win.segs,
+                                           kv_group, &win);
+}
+
 // Merges the `splits` KV-slice partials of one split tile: out = (sum_i w_i O_i) / (sum_i w_i l_i), w_i = 2^((m_i - m) c).
 // One CTA per (split tile, query row), thread = output column.
-template <bool kPacked>
+template <bool kPacked, bool kWin = false>
 __device__ __forceinline__ void attention_combine_body(const float* __restrict__ part_ws, __nv_bfloat16* __restrict__ out, int H,
                                                        int Lq, int d_model, float scale_log2, int n_full, int splits,
-                                                       const AttnSegs* segs) {
+                                                       const AttnSegs* segs, const AttnWin* win = nullptr) {
     int n_qt = (Lq + 127) / 128;
     const int st = blockIdx.x, r = blockIdx.y, c = threadIdx.x;
     pdl_launch_dependents();
@@ -311,6 +338,10 @@ __device__ __forceinline__ void attention_combine_body(const float* __restrict__
             if (tile >= segs->tile0[i]) seg = i;
         seg0 = segs->start[seg];
         Lq = segs->start[seg + 1] - seg0;
+        if constexpr (kWin) {
+            seg0 = win->out0[seg];  // output rows of the window
+            Lq = win->nq[seg];
+        }
         n_qt = (Lq + 127) / 128;
         tl = tile - segs->tile0[seg];
     }
@@ -340,6 +371,12 @@ __global__ void __launch_bounds__(128)
 attention_packed_combine_kernel(const float* __restrict__ part_ws, __nv_bfloat16* __restrict__ out, int H, int d_model,
                                 float scale_log2, int n_full, int splits, const __grid_constant__ AttnSegs segs) {
     attention_combine_body<true>(part_ws, out, H, 0, d_model, scale_log2, n_full, splits, &segs);
+}
+
+__global__ void __launch_bounds__(128)
+attention_packed_window_combine_kernel(const float* __restrict__ part_ws, __nv_bfloat16* __restrict__ out, int H, int d_model,
+                                       float scale_log2, int n_full, int splits, const __grid_constant__ AttnWin win) {
+    attention_combine_body<true, true>(part_ws, out, H, 0, d_model, scale_log2, n_full, splits, &win.segs, &win);
 }
 
 // KV-slice partials of the split tail: one buffer per (device, stream), grown on demand
@@ -446,24 +483,37 @@ static int attention_launch(const __nv_bfloat16* q, const __nv_bfloat16* k, cons
     return 0;
 }
 
+// win_lo / win_hi (host, both null or both set): sequence s queries its rows [win_lo[s], win_hi[s]) only, and `out` is compact
 template <int kBKV>
 static int attention_packed_launch(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* vt, __nv_bfloat16* out,
-                                   const SegTable& segs, int H, int Lpad, float scale, cudaStream_t stream, int Hkv) {
+                                   const SegTable& segs, int H, int Lpad, float scale, cudaStream_t stream, int Hkv,
+                                   const int* win_lo, const int* win_hi) {
     constexpr int kAttnSmem = AttnCfg<kBKV>::kSmem;
     if (segs.n <= 0 || segs.n > kMaxSegs || H <= 0) return set_error("attention_packed: %d sequences (1 to %d)", segs.n, kMaxSegs);
     if (Hkv <= 0) Hkv = H;
     if (Hkv > H || H % Hkv) return set_error("attention_packed: n_kv_heads=%d must divide n_heads=%d", Hkv, H);
     if (Lpad % 8) return set_error("attention_packed: Lpad must be a multiple of 8");
-    AttnSegs as{};
+    if (!win_lo != !win_hi) return set_error("attention_packed: give both window bounds or neither");
+    const bool windowed = win_lo != nullptr;
+    AttnWin aw{};
+    AttnSegs& as = aw.segs;
     as.n = segs.n;
     double work = 0;
+    int Mq = 0;  // windowed: rows of the compact output
     for (int s = 0; s <= segs.n; ++s) {
         as.start[s] = segs.start[s];
         if (s == segs.n) break;
         const int len = segs.start[s + 1] - segs.start[s];
         if (len <= 0 || len > Lpad) return set_error("attention_packed: sequence %d has length %d (Lpad %d)", s, len, Lpad);
-        as.tile0[s + 1] = as.tile0[s] + (len + 127) / 128 * H;
-        work += 4.0 * H * (double)len * len * 128;
+        const int lo = windowed ? win_lo[s] : 0, hi = windowed ? win_hi[s] : len;
+        if (lo < 0 || lo >= hi || hi > len)
+            return set_error("attention_packed: sequence %d of length %d has the row window [%d, %d)", s, len, lo, hi);
+        aw.q0[s] = lo;
+        aw.nq[s] = hi - lo;
+        aw.out0[s] = Mq;
+        Mq += hi - lo;
+        as.tile0[s + 1] = as.tile0[s] + (hi - lo + 127) / 128 * H;
+        work += 4.0 * H * (double)(hi - lo) * len * 128;
     }
     const int M = segs.start[segs.n], tiles = as.tile0[segs.n], d_model = H * 128, d_kv = Hkv * 128;
     CUtensorMap tmQ, tmK, tmVt;
@@ -483,6 +533,17 @@ static int attention_packed_launch(const __nv_bfloat16* q, const __nv_bfloat16* 
     const float scale_log2 = scale * 1.4426950408889634f;
     const bool pdl = pdl_mode() != 0;
     LaunchScope ls(LK_ATTN, work, stream);
+    if (windowed) {
+        auto kernel = Hkv != H ? attention_packed_window_kernel<kBKV, true> : attention_packed_window_kernel<kBKV, false>;
+        static unsigned long long attr_set_win[2] = {0, 0};
+        if (attn_smem_attr(kernel, kAttnSmem, attr_set_win[Hkv != H])) return -1;
+        MMDP_CUDA(launch_ex(kernel, dim3(grid), dim3(kAttnThreads), kAttnSmem, stream, pdl, false, tmQ, tmK, tmVt, out, H, d_model,
+                            scale_log2, n_full, splits, part_ws, aw, H / Hkv));
+        if (n_split > 0)
+            MMDP_CUDA(launch_ex(attention_packed_window_combine_kernel, dim3(n_split, 128), dim3(128), 0, stream, pdl, false,
+                                (const float*)part_ws, out, H, d_model, scale_log2, n_full, splits, aw));
+        return 0;
+    }
     if (Hkv != H) {
         static unsigned long long attr_set_gqa = 0;
         if (attn_smem_attr(attention_packed_gqa_kernel<kBKV>, kAttnSmem, attr_set_gqa)) return -1;
@@ -509,11 +570,12 @@ int attention_fwd(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfl
 }
 
 int attention_packed_fwd(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* vt, __nv_bfloat16* out,
-                         const SegTable& segs, int H, int Lpad, float scale, cudaStream_t stream, int Hkv) {
+                         const SegTable& segs, int H, int Lpad, float scale, cudaStream_t stream, int Hkv, const int* win_lo,
+                         const int* win_hi) {
     const int version = opt(OPT_ATTN_VERSION);
-    if (version == 7) return attention_packed_launch<64>(q, k, vt, out, segs, H, Lpad, scale, stream, Hkv);
+    if (version == 7) return attention_packed_launch<64>(q, k, vt, out, segs, H, Lpad, scale, stream, Hkv, win_lo, win_hi);
     if (version != 6) return set_error("attention: unknown kernel generation %d (6 or 7)", version);
-    return attention_packed_launch<128>(q, k, vt, out, segs, H, Lpad, scale, stream, Hkv);
+    return attention_packed_launch<128>(q, k, vt, out, segs, H, Lpad, scale, stream, Hkv, win_lo, win_hi);
 }
 
 }  // namespace mmdp

@@ -170,9 +170,12 @@ void set_gemm_splitk_mode(int mode);
 int attention_fwd(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* vt, __nv_bfloat16* out, int B,
                   int H, int L, int Lpad, float scale, cudaStream_t stream, int Lq = 0, int Hkv = 0);
 // packed variable-length batch: q / out [segs.start[n], H * 128], k [segs.start[n], Hkv * 128], vt [segs.n, Hkv, 128, Lpad];
-// columns [L_s, Lpad) of sequence s's V^T block must be finite zeros
+// columns [L_s, Lpad) of sequence s's V^T block must be finite zeros.
+// win_lo / win_hi (host arrays, both or neither): sequence s computes its query rows [win_lo[s], win_hi[s]) only, against all of
+// its keys, and out holds the windows end to end (sum of hi - lo rows); 0 <= lo < hi <= L_s
 int attention_packed_fwd(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* vt, __nv_bfloat16* out,
-                         const SegTable& segs, int H, int Lpad, float scale, cudaStream_t stream, int Hkv = 0);
+                         const SegTable& segs, int H, int Lpad, float scale, cudaStream_t stream, int Hkv = 0,
+                         const int* win_lo = nullptr, const int* win_hi = nullptr);
 
 // err (nullable): device int, bit 0 is raised when an id is outside [0, vocab) (the kernel then reads row 0)
 int embed_rows(const int64_t* ids, const __nv_bfloat16* wte, __nv_bfloat16* x, int M, int d, int64_t vocab,

@@ -16,6 +16,11 @@ Requests with fewer steps drop out. A set of more than `max_batch` sequences run
 The sampling stays per request: each draws from its own generator in the order generate_ti2ti does, so the draws of one
 request do not depend on its neighbours. Still-masked image tokens are drawn from the global CPU RNG after the loop, in request
 order, like sequential calls would.
+
+`interleave_generate_batch(model, requests)` does the same for variant M's `MMadaModelLM.interleave_generate`: one packed forward
+per global step over the cond and uncond sequences of every active request, then each request's text step and, on its image
+steps, its image step (`interleave_text_step` / `interleave_image_step`, the code interleave_generate runs). Each sequence gets
+the last-block row window interleave_generate would give it.
 """
 from __future__ import annotations
 
@@ -28,9 +33,10 @@ from ..schedule import get_num_transfer_tokens, image_generation_step_indices
 from .parallel_generator import (DenoiseState, _Noise, check_request, extract_results, generate_ti2ti, image_sample,
                                  text_sample, uncond_inputs)
 
-__all__ = ["generate_ti2ti_batch", "batch_schedule", "packed_chunks"]
+__all__ = ["generate_ti2ti_batch", "interleave_generate_batch", "batch_schedule", "packed_chunks"]
 
 _SIGNATURE = inspect.signature(generate_ti2ti)
+_MAX_SEGS = 64  # sequences of one packed forward (kMaxSegs in csrc/mmdp_internal.h)
 
 
 def batch_schedule(text_steps: Sequence[int], timesteps: Sequence[int]) -> List[tuple]:
@@ -85,19 +91,23 @@ def _bind(model, requests) -> List[dict]:
     return args
 
 
-def _packed_forward(model, seqs: list, col0_b: int, ncols_b: int) -> list:
+def _packed_forward(model, seqs: list, col0_b: int, ncols_b: int, windows=None) -> list:
     """Packed forwards over seqs = [(ids [L] cuda int64, text rows int32 or None, image rows int32 or None)], max_batch sequences
-    per forward. Returns [(text logits [n_a, V] or None, image logits [n_b, ncols_b] or None)] per sequence (views)."""
+    per forward. windows (optional): the last-block row window (lo, hi) or None of every sequence. Returns [(text logits [n_a, V]
+    or None, image logits [n_b, ncols_b] or None)] per sequence (views)."""
     outs = []
-    for chunk in packed_chunks(len(seqs), model.max_batch):
+    for chunk in packed_chunks(len(seqs), min(model.max_batch, _MAX_SEGS)):
         part = [seqs[i] for i in chunk]
         lens = [s[0].numel() for s in part]
         offs = [sum(lens[:j]) for j in range(len(part))]
         ra = [s[1] + o for s, o in zip(part, offs) if s[1] is not None]
         rb = [s[2] + o for s, o in zip(part, offs) if s[2] is not None]
+        win = None
+        if windows is not None and any(windows[i] is not None for i in chunk):
+            win = [windows[i] for i in chunk]
         out_a, out_b = model.forward_rows_packed(torch.cat([s[0] for s in part]), lens,
                                                  rows_a=torch.cat(ra) if ra else None, rows_b=torch.cat(rb) if rb else None,
-                                                 col0_b=col0_b, ncols_b=ncols_b)
+                                                 col0_b=col0_b, ncols_b=ncols_b, row_windows=win)
         oa = ob = 0
         for s in part:
             va = vb = None
@@ -162,3 +172,76 @@ def generate_ti2ti_batch(model, requests: Sequence[dict]) -> list:
         image_tokens, text, _ = extract_results(st, final, a["tokenizer"], a["text_vocab_size"], a["codebook_size"])
         results.append((image_tokens, text))
     return results
+
+
+def _bind_m(model, requests) -> List[dict]:
+    """Every request's interleave_generate arguments with its defaults, checked before anything runs on the device."""
+    from ..mmada import MMadaModelLM, interleave_layout
+    if not requests:
+        raise ValueError("interleave_generate_batch needs at least one request")
+    sig = inspect.signature(MMadaModelLM.interleave_generate)
+    args, seen = [], set()
+    for i, r in enumerate(requests):
+        a = sig.bind(model, **r)
+        a.apply_defaults()
+        a = dict(a.arguments)
+        a.update(a.pop("kwargs"))
+        if not (a["text_cfg"] or a["image_cfg"]):
+            raise ValueError(f"request {i}: text_cfg and image_cfg cannot be both 0")
+        if a["remasking"] != "low_confidence":
+            raise NotImplementedError(a["remasking"])
+        g = a["generator"]
+        if not isinstance(g, torch.Generator):
+            raise ValueError(f"request {i}: every request needs its own torch.Generator (got {g!r}); draws from a shared or "
+                             "the global generator would interleave differently from sequential calls")
+        if id(g) in seen:
+            raise ValueError(f"request {i} shares its generator with an earlier request; each request needs its own")
+        seen.add(id(g))
+        if a["text_temperature"] != 0:
+            raise ValueError(f"request {i}: text_temperature={a['text_temperature']} draws its Gumbel noise from the device's global "
+                             "RNG, which sequential calls consume request after request; a batch cannot reproduce that order")
+        lay = interleave_layout(a["config"], a.get("uni_prompting"), a["input_ids"], a["uncond_input_ids"], a["text_steps"],
+                                a["image_steps"])
+        if lay["L"] > model.max_seq_len:
+            raise ValueError(f"request {i}: sequence of {lay['L']} tokens exceeds the model's max_seq_len={model.max_seq_len}")
+        if not lay["img_idx"]:
+            raise RuntimeError(f"request {i}: no image step was scheduled (the reference would hit an undefined `sampled_ids`)")
+        for key, name in (("tvoc", "len(uni_prompting.text_tokenizer)"), ("C", "codebook_size")):
+            if args and lay[key] != args[0]["_layout"][key]:
+                raise ValueError(f"all requests of a batch share {name} (request {i}: {lay[key]}, request 0: {args[0]['_layout'][key]})")
+        a["_layout"] = lay
+        args.append(a)
+    if not hasattr(model, "forward_rows_packed"):
+        raise TypeError("interleave_generate_batch needs a model with packed forwards (mmada_parallel_b200.mmada.MMadaModelLM)")
+    return args
+
+
+@torch.no_grad()
+def interleave_generate_batch(model, requests: Sequence[dict]) -> list:
+    """Runs the variant-M interleave_generate requests (dicts of its keyword arguments) together and returns their results in
+    request order: `[model.interleave_generate(**r) for r in requests]`, the (image_ids [1, num_vq_tokens], text_ids
+    [1, max_seq_length]) tensors, with every request's generator left in the same state. Each request needs its own
+    torch.Generator and text_temperature=0; all share the text vocabulary size and the codebook size. Argument errors raise
+    before any forward."""
+    from ..mmada import InterleaveState, interleave_image_step, interleave_text_step
+    args = _bind_m(model, requests)
+    col0, ncols = args[0]["_layout"]["tvoc"], args[0]["_layout"]["C"]
+    states = [InterleaveState(model, **{k: v for k, v in a.items() if k not in ("self", "_layout")}) for a in args]
+    steps = [a["text_steps"] for a in args]
+    for g, (active, img) in enumerate(batch_schedule(steps, [a["image_steps"] for a in args])):
+        img_set = set(img)
+        # one packed forward (:172) over [cond; uncond] of every active request, each sequence with its own row window
+        seqs, windows = [], []
+        for i in active:
+            st = states[i]
+            rows_text = st.rows_text[:st.max_seq]
+            for b in range(2):
+                seqs.append((st.both[b], rows_text, st.pos if i in img_set else None))
+                windows.append(st.window(g))
+        outs = _packed_forward(model, seqs, col0, ncols, windows)
+        for j, i in enumerate(active):
+            (ta, ia), (tu, iu) = outs[2 * j], outs[2 * j + 1]
+            interleave_text_step(states[i], g, ta, tu)
+            if i in img_set:
+                interleave_image_step(states[i], g, ia, iu)
+    return [st.results() for st in states]

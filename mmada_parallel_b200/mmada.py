@@ -51,91 +51,17 @@ class MMadaModelLM(LLaDAForMultiModalGeneration):
         image_temperature: float = 1.0,
         **kwargs,
     ):
-        if not (text_cfg or image_cfg):
-            raise ValueError("text_cfg and image_cfg cannot be both 0")                      # :181-182
-        if remasking != "low_confidence":
-            raise NotImplementedError(remasking)
-        uni_prompting = kwargs.get("uni_prompting", None)
-        _text_noise = kwargs.get("_text_noise", None)   # tests: injects the fp64 uniform noise instead of the global-RNG draw
-        dev = self.device
-        mask_id = int(self.config.mask_token_id)
-        n_vq = int(config.model.mmada.num_vq_tokens)
-        C = int(config.model.mmada.codebook_size)
-        max_seq = int(config.dataset.preprocessing.max_seq_length)
-        tvoc = len(uni_prompting.text_tokenizer)
-        inp = input_ids.to(device=dev, dtype=torch.int64).unsqueeze(0)
-        unc = uncond_input_ids.to(device=dev, dtype=torch.int64).unsqueeze(0)
-        full = lambda n, v: torch.full((1, n), int(v), dtype=torch.int64, device=dev)
-        out_ids = torch.cat([full(1, reserved_token_mapping["<|soi|>"]), full(n_vq, mask_id),
-                             full(1, reserved_token_mapping["<|eoi|>"]), full(1, uni_prompting.text_tokenizer.bos_token_id),
-                             full(max_seq - 1, mask_id)], dim=1)                               # :142-148
-        P = inp.shape[1]
-        L = P + out_ids.shape[1]
-        if unc.shape[1] != P:
-            raise ValueError("cond and uncond prompts must have equal length (padding is not masked, SURVEY App. A3)")
-        both = torch.empty((2, L), dtype=torch.int64, device=dev)                             # [cond; uncond] id buffer
-        both[0, :P] = inp[0]
-        both[1, :P] = unc[0]
-        both[:, P:] = out_ids
-        num_transfer = get_num_transfer_tokens_m(max_seq - 1, text_steps)                     # bos is not a mask
-        img_idx = set(image_generation_step_indices(text_steps, image_steps))
-        V = self.vocab_rows
-        t0 = L - max_seq
-        rows_text = torch.cat([torch.arange(t0, L, dtype=torch.int32, device=dev),
-                               torch.arange(L + t0, 2 * L, dtype=torch.int32, device=dev)])
-        pos = torch.arange(P + 1, P + 1 + n_vq, dtype=torch.int32, device=dev)
-        rows_img = torch.cat([pos, pos + L])
-        text_logits = torch.empty((2 * max_seq, V), dtype=torch.bfloat16, device=dev)
-        img_logits = torch.empty((2 * n_vq, C), dtype=torch.bfloat16, device=dev)
-        x0_ws = torch.empty(max_seq, dtype=torch.int64, device=dev)
-        conf_ws = torch.empty(max_seq, dtype=torch.float64, device=dev)
-        sampled_ws = torch.zeros(n_vq, dtype=torch.int32, device=dev)
-        selp_ws = torch.empty(n_vq, dtype=torch.float32, device=dev)
-        unk_ws = torch.empty(n_vq, dtype=torch.uint8, device=dev)
-        noise = _Noise(generator, dev)
-        any_image_step = False
-        # positions whose logits are read, per batch row: the last block computes its attention output / MLP for them only
-        # (model.forward_rows, row_window; long sequences only - the tiny parity models keep one fixed kernel schedule)
-        win_text, win_img = ((t0, L), (P + 1, L)) if L >= 1024 else (None, None)
+        st = InterleaveState(self, input_ids, uncond_input_ids, text_cfg, image_cfg, noise_schedule, text_steps, image_steps,
+                             reserved_token_mapping, generator, config, remasking, text_temperature, image_temperature, **kwargs)
         for i in range(text_steps):
-            is_img = i in img_idx
-            self.forward_rows(both, rows_a=rows_text, out_a=text_logits, rows_b=rows_img if is_img else None,
-                              col0_b=tvoc, ncols_b=C, out_b=img_logits if is_img else None,
-                              row_window=win_img if is_img else win_text)                       # :172
-            # text step on the CFG-mixed logits (:179-209); only the cond row's ids change ...
-            if text_temperature != 0:
-                # add_gumbel_noise (:49-60): fp64 uniform noise of the text-logits shape from the GLOBAL RNG of the logits'
-                # device - the same call the reference makes on a GPU, so the same Philox stream is consumed
-                u64 = (_text_noise(i, (1, max_seq, V)) if _text_noise is not None
-                       else torch.rand((1, max_seq, V), dtype=torch.float64, device=dev)).to(dev).contiguous()
-                check(lib.mmdp_text_step_gumbel64(ptr(text_logits), text_logits.data_ptr() + max_seq * V * 2, V, max_seq, V,
-                                                  float(text_cfg), ptr(u64), V, float(text_temperature), both.data_ptr() + t0 * 8,
-                                                  mask_id, int(num_transfer[i]), ptr(x0_ws), ptr(conf_ws), stream_ptr()))
-            else:
-                check(lib.mmdp_text_step(ptr(text_logits), text_logits.data_ptr() + max_seq * V * 2, V, max_seq, V,
-                                         float(text_cfg), None, 0, 0.0, both.data_ptr() + t0 * 8, mask_id,
-                                         int(num_transfer[i]), ptr(x0_ws), ptr(conf_ws), stream_ptr()))
-            # ... and the uncond row shares the generated suffix (:166-169)
-            both[1, P:] = both[0, P:]
-            if not is_img:
-                continue
-            any_image_step = True
-            q = noise.exponential((n_vq, C))                                                    # multinomial (:222)
-            ratio = 1.0 * (i + 1) / text_steps
-            temp = image_temperature * (1.0 - ratio)                                            # :236
-            # gumbel_noise(): torch.zeros_like(t).uniform_(0, 1, generator=generator)  (M/models/sampling.py:14-15)
-            un = torch.zeros((1, n_vq), dtype=torch.bfloat16, device=noise.gdev).uniform_(0, 1, generator=generator).to(dev)
-            check(lib.mmdp_image_step(1, ptr(img_logits), img_logits.data_ptr() + n_vq * C * 2, None, C, n_vq, C,
-                                      float(image_cfg), float(1 + image_cfg), ptr(q), ptr(un), float(temp),
-                                      scheduled_mask_len(n_vq, i, text_steps, noise_schedule), ptr(both), ptr(pos),
-                                      mask_id, tvoc, ptr(sampled_ws), ptr(selp_ws), ptr(unk_ws), None, None, None,
-                                      stream_ptr()))
-            both[1, P:] = both[0, P:]
-        if not any_image_step:
-            raise RuntimeError("no image step was scheduled (the reference would hit an undefined `sampled_ids`)")
-        return_image_ids = sampled_ws.to(torch.int64).unsqueeze(0)
-        return_text_ids = both[0:1, -max_seq:].clone()
-        return return_image_ids, return_text_ids
+            is_img = i in st.img_idx
+            self.forward_rows(st.both, rows_a=st.rows_text, out_a=st.text_logits, rows_b=st.rows_img if is_img else None,
+                              col0_b=st.tvoc, ncols_b=st.C, out_b=st.img_logits if is_img else None,
+                              row_window=st.window(i))                                           # :172
+            interleave_text_step(st, i, st.text_logits[:st.max_seq], st.text_logits[st.max_seq:])
+            if is_img:
+                interleave_image_step(st, i, st.img_logits[:st.n_vq], st.img_logits[st.n_vq:])
+        return st.results()
 
     @torch.no_grad()
     def mmu_generate(self, idx=None, input_embeddings=None, max_new_tokens=128, steps=128, block_length=128, temperature=0.0,
@@ -280,3 +206,118 @@ class MMadaModelLM(LLaDAForMultiModalGeneration):
             caller_ids.copy_(ids.to(caller_ids.device))                                                    # in-place update, like the reference
         self.raise_device_errors()
         return sampled_ws.to(torch.int64)
+
+
+def interleave_layout(config, uni_prompting, input_ids, uncond_input_ids, text_steps: int, image_steps: int) -> dict:
+    """Host-side shape of one interleave_generate request, checked before anything touches the device: prompt length P, sequence
+    length L = P + num_vq_tokens + max_seq_length + 2, text start t0, text vocabulary size and codebook size."""
+    n_vq = int(config.model.mmada.num_vq_tokens)
+    max_seq = int(config.dataset.preprocessing.max_seq_length)
+    P = int(input_ids.shape[-1])
+    if int(uncond_input_ids.shape[-1]) != P:
+        raise ValueError("cond and uncond prompts must have equal length (padding is not masked, SURVEY App. A3)")
+    L = P + n_vq + max_seq + 2                                                                   # soi, vq, eoi, bos, text masks
+    return dict(n_vq=n_vq, max_seq=max_seq, P=P, L=L, t0=L - max_seq, C=int(config.model.mmada.codebook_size),
+                tvoc=len(uni_prompting.text_tokenizer),
+                img_idx=set(image_generation_step_indices(text_steps, image_steps)))
+
+
+class InterleaveState:
+    """Device-resident state of one interleave_generate request (modeling_mmada.py:118-248): the CFG id buffer [cond; uncond],
+    its logits rows, the sampling workspaces and the request's noise source. `interleave_generate` and
+    generators/batch.py::interleave_generate_batch advance it with `interleave_text_step` / `interleave_image_step`."""
+
+    def __init__(self, model, input_ids, uncond_input_ids, text_cfg, image_cfg, noise_schedule, text_steps, image_steps,
+                 reserved_token_mapping, generator, config, remasking, text_temperature, image_temperature, **kwargs):
+        if not (text_cfg or image_cfg):
+            raise ValueError("text_cfg and image_cfg cannot be both 0")                      # :181-182
+        if remasking != "low_confidence":
+            raise NotImplementedError(remasking)
+        uni_prompting = kwargs.get("uni_prompting", None)
+        self._text_noise = kwargs.get("_text_noise", None)  # tests: injects the fp64 uniform noise instead of the global-RNG draw
+        lay = interleave_layout(config, uni_prompting, input_ids, uncond_input_ids, text_steps, image_steps)
+        self.n_vq, self.max_seq, self.C, self.tvoc, self.img_idx = lay["n_vq"], lay["max_seq"], lay["C"], lay["tvoc"], lay["img_idx"]
+        self.text_cfg, self.image_cfg, self.noise_schedule = float(text_cfg), float(image_cfg), noise_schedule
+        self.text_steps, self.text_temperature, self.image_temperature = text_steps, text_temperature, image_temperature
+        self.generator = generator
+        dev = self.dev = model.device
+        self.mask_id = mask_id = int(model.config.mask_token_id)
+        n_vq, max_seq = self.n_vq, self.max_seq
+        inp = input_ids.to(device=dev, dtype=torch.int64).unsqueeze(0)
+        unc = uncond_input_ids.to(device=dev, dtype=torch.int64).unsqueeze(0)
+        full = lambda n, v: torch.full((1, n), int(v), dtype=torch.int64, device=dev)
+        out_ids = torch.cat([full(1, reserved_token_mapping["<|soi|>"]), full(n_vq, mask_id),
+                             full(1, reserved_token_mapping["<|eoi|>"]), full(1, uni_prompting.text_tokenizer.bos_token_id),
+                             full(max_seq - 1, mask_id)], dim=1)                               # :142-148
+        P = self.P = inp.shape[1]
+        L = self.L = P + out_ids.shape[1]
+        both = self.both = torch.empty((2, L), dtype=torch.int64, device=dev)                  # [cond; uncond] id buffer
+        both[0, :P] = inp[0]
+        both[1, :P] = unc[0]
+        both[:, P:] = out_ids
+        self.num_transfer = get_num_transfer_tokens_m(max_seq - 1, text_steps)                # bos is not a mask
+        V = model.vocab_rows
+        t0 = self.t0 = L - max_seq
+        self.rows_text = torch.cat([torch.arange(t0, L, dtype=torch.int32, device=dev),
+                                    torch.arange(L + t0, 2 * L, dtype=torch.int32, device=dev)])
+        self.pos = torch.arange(P + 1, P + 1 + n_vq, dtype=torch.int32, device=dev)
+        self.rows_img = torch.cat([self.pos, self.pos + L])
+        self.text_logits = torch.empty((2 * max_seq, V), dtype=torch.bfloat16, device=dev)
+        self.img_logits = torch.empty((2 * n_vq, self.C), dtype=torch.bfloat16, device=dev)
+        self.x0_ws = torch.empty(max_seq, dtype=torch.int64, device=dev)
+        self.conf_ws = torch.empty(max_seq, dtype=torch.float64, device=dev)
+        self.sampled_ws = torch.zeros(n_vq, dtype=torch.int32, device=dev)
+        self.selp_ws = torch.empty(n_vq, dtype=torch.float32, device=dev)
+        self.unk_ws = torch.empty(n_vq, dtype=torch.uint8, device=dev)
+        self.noise = _Noise(generator, dev)
+        self.any_image_step = False
+        # positions whose logits are read, per batch row: the last block computes its attention output / MLP for them only
+        # (model.forward_rows, row_window; long sequences only - the tiny parity models keep one fixed kernel schedule)
+        self.win_text, self.win_img = ((t0, L), (P + 1, L)) if L >= 1024 else (None, None)
+
+    def window(self, i: int):
+        """The last-block row window of step i (per sequence): the text rows, and on image steps the image rows too."""
+        return self.win_img if i in self.img_idx else self.win_text
+
+    def results(self):
+        if not self.any_image_step:
+            raise RuntimeError("no image step was scheduled (the reference would hit an undefined `sampled_ids`)")
+        return_image_ids = self.sampled_ws.to(torch.int64).unsqueeze(0)
+        return_text_ids = self.both[0:1, -self.max_seq:].clone()
+        return return_image_ids, return_text_ids
+
+
+def interleave_text_step(st: InterleaveState, i: int, cond: torch.Tensor, uncond: torch.Tensor) -> None:
+    """Step i's text step on the CFG-mixed logits (:179-209): cond / uncond [max_seq, V] are the text rows' logits of the two
+    sequences. Only the cond row's ids change; the uncond row then shares the generated suffix (:166-169)."""
+    max_seq, V = st.max_seq, cond.shape[1]
+    if st.text_temperature != 0:
+        # add_gumbel_noise (:49-60): fp64 uniform noise of the text-logits shape from the GLOBAL RNG of the logits'
+        # device - the same call the reference makes on a GPU, so the same Philox stream is consumed
+        u64 = (st._text_noise(i, (1, max_seq, V)) if st._text_noise is not None
+               else torch.rand((1, max_seq, V), dtype=torch.float64, device=st.dev)).to(st.dev).contiguous()
+        check(lib.mmdp_text_step_gumbel64(ptr(cond), ptr(uncond), V, max_seq, V, st.text_cfg, ptr(u64), V,
+                                          float(st.text_temperature), st.both.data_ptr() + st.t0 * 8, st.mask_id,
+                                          int(st.num_transfer[i]), ptr(st.x0_ws), ptr(st.conf_ws), stream_ptr()))
+    else:
+        check(lib.mmdp_text_step(ptr(cond), ptr(uncond), V, max_seq, V, st.text_cfg, None, 0, 0.0,
+                                 st.both.data_ptr() + st.t0 * 8, st.mask_id, int(st.num_transfer[i]), ptr(st.x0_ws),
+                                 ptr(st.conf_ws), stream_ptr()))
+    st.both[1, st.P:] = st.both[0, st.P:]
+
+
+def interleave_image_step(st: InterleaveState, i: int, cond: torch.Tensor, uncond: torch.Tensor) -> None:
+    """Step i's image step (:211-240) on cond / uncond [n_vq, codebook_size], the image rows' codebook logits; draws the
+    multinomial's exponentials, then the re-masking noise, from the request's generator."""
+    n_vq, C = st.n_vq, st.C
+    st.any_image_step = True
+    q = st.noise.exponential((n_vq, C))                                                         # multinomial (:222)
+    ratio = 1.0 * (i + 1) / st.text_steps
+    temp = st.image_temperature * (1.0 - ratio)                                                 # :236
+    # gumbel_noise(): torch.zeros_like(t).uniform_(0, 1, generator=generator)  (M/models/sampling.py:14-15)
+    un = torch.zeros((1, n_vq), dtype=torch.bfloat16, device=st.noise.gdev).uniform_(0, 1, generator=st.generator).to(st.dev)
+    check(lib.mmdp_image_step(1, ptr(cond), ptr(uncond), None, C, n_vq, C, st.image_cfg, float(1 + st.image_cfg), ptr(q), ptr(un),
+                              float(temp), scheduled_mask_len(n_vq, i, st.text_steps, st.noise_schedule), ptr(st.both),
+                              ptr(st.pos), st.mask_id, st.tvoc, ptr(st.sampled_ws), ptr(st.selp_ws), ptr(st.unk_ws), None, None,
+                              None, stream_ptr()))
+    st.both[1, st.P:] = st.both[0, st.P:]

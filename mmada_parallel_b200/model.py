@@ -284,7 +284,7 @@ class LLaDAForMultiModalGeneration:
         if flags.value & 2:
             raise IndexError("a logits row index is outside [0, batch * seq_len)")
         if flags.value & 4:
-            raise IndexError("a logits row index is outside the row window given to forward_rows")
+            raise IndexError("a logits row index is outside the row window given to forward_rows / forward_rows_packed")
 
     # ------------------------------------------------------------------------------------------------------------
     # forward
@@ -342,12 +342,16 @@ class LLaDAForMultiModalGeneration:
 
     def forward_rows_packed(self, ids_packed: torch.Tensor, seq_lens, rows_a: Optional[torch.Tensor] = None,
                             rows_b: Optional[torch.Tensor] = None, col0_b: int = 0, ncols_b: int = 0,
-                            out_a: Optional[torch.Tensor] = None, out_b: Optional[torch.Tensor] = None):
+                            out_a: Optional[torch.Tensor] = None, out_b: Optional[torch.Tensor] = None, row_windows=None):
         """One forward over a packed batch of several sequences of different lengths: ids_packed [sum(seq_lens)] (cuda int64) holds
         the sequences end to end. Each sequence is computed as if it were alone (attention stays inside it, positions restart at
         0), so its logits equal those of its own `forward_rows`. rows_* are int32 packed row indices (offset of the sequence +
         position). Returns (logits_a [n_a, V] or None, logits_b [n_b, ncols_b] or None), like `forward_rows`.
-        At most `max_batch` sequences, each at most `max_seq_len` long (ValueError otherwise)."""
+        At most `max_batch` sequences, each at most `max_seq_len` long (ValueError otherwise).
+        row_windows: one (lo, hi) or None per sequence, the `row_window` of its own `forward_rows`: every requested row of that
+        sequence is a position in [lo, hi), and the last block computes its attention output and MLP for those positions only.
+        None stands for the whole sequence. A malformed window raises ValueError; a requested row outside its window raises
+        IndexError at the next raise_device_errors()."""
         lens = [int(x) for x in seq_lens]
         if not lens or len(lens) > self.max_batch:
             raise ValueError(f"a packed forward takes 1 to max_batch={self.max_batch} sequences, got {len(lens)}")
@@ -355,6 +359,16 @@ class LLaDAForMultiModalGeneration:
             raise ValueError(f"packed sequence lengths must lie in [1, max_seq_len={self.max_seq_len}], got {lens}")
         if ids_packed.numel() != sum(lens):
             raise ValueError(f"ids_packed holds {ids_packed.numel()} tokens, the sequence lengths add up to {sum(lens)}")
+        c_lo = c_hi = None
+        if row_windows is not None:
+            if len(row_windows) != len(lens):
+                raise ValueError(f"row_windows has {len(row_windows)} entries for {len(lens)} sequences")
+            wins = [(0, L) if w is None else (int(w[0]), int(w[1])) for w, L in zip(row_windows, lens)]
+            for (lo, hi), L in zip(wins, lens):
+                if not 0 <= lo < hi <= L:
+                    raise ValueError(f"row window ({lo}, {hi}) does not satisfy 0 <= lo < hi <= {L} (its sequence's length)")
+            c_lo = (C.c_int32 * len(lens))(*[w[0] for w in wins])
+            c_hi = (C.c_int32 * len(lens))(*[w[1] for w in wins])
         ids = ids_packed.to(device=self.device, dtype=torch.int64).contiguous()
         n_a = 0 if rows_a is None else rows_a.numel()
         n_b = 0 if rows_b is None else rows_b.numel()
@@ -363,6 +377,7 @@ class LLaDAForMultiModalGeneration:
         if n_b and out_b is None:
             out_b = torch.empty((n_b, ncols_b), dtype=torch.bfloat16, device=self.device)
         c_lens = (C.c_int32 * len(lens))(*lens)
-        check(lib.mmdp_model_forward_packed(self._h, ptr(ids), len(lens), c_lens, ptr(rows_a), n_a, ptr(out_a) if n_a else None,
-                                            ptr(rows_b), n_b, col0_b, ncols_b, ptr(out_b) if n_b else None, stream_ptr()))
+        check(lib.mmdp_model_forward_packed_window(self._h, ptr(ids), len(lens), c_lens, c_lo, c_hi, ptr(rows_a), n_a,
+                                                   ptr(out_a) if n_a else None, ptr(rows_b), n_b, col0_b, ncols_b,
+                                                   ptr(out_b) if n_b else None, stream_ptr()))
         return (out_a if n_a else None), (out_b if n_b else None)
