@@ -356,6 +356,8 @@ MMDP_API int mmdp_tp_reduce_norm(const float* recv_local, int rows_per_rank, int
 MMDP_API int mmdp_gemm_f32_scatter(const uint16_t* A, int lda, const uint16_t* W, int ldw, int M, int N, int K, float* const* recv,
                           int n_ranks, int rows_per_rank, int slot, void* stream) {
     if (!recv || n_ranks < 1 || n_ranks > 8) return set_error("mmdp_gemm_f32_scatter: bad rank layout");
+    // the receive buffers hold n_ranks slots: a slot past them would be pushed beyond the owner's buffer
+    if (slot < 0 || slot >= n_ranks) return set_error("mmdp_gemm_f32_scatter: slot %d outside [0, %d)", slot, n_ranks);
     if (rows_per_rank <= 0 || (M + rows_per_rank - 1) / rows_per_rank > n_ranks) return set_error("mmdp_gemm_f32_scatter: M does not fit n_ranks x rows_per_rank");
     GemmScatter sc{};
     for (int r = 0; r < n_ranks; ++r) sc.dst[r] = recv[r];
