@@ -96,14 +96,18 @@ MMDP_API int mmdp_tp_reduce_norm(const float* recv_local, int rows_per_rank, int
  * per layer left a TP=8 rank CPU-bound): embedding of this rank's rows, norm + broadcast, then per layer column-parallel QKV+RoPE,
  * attention on the local heads, row-parallel attn_out pushed to the owners, reduce + residual + ff_norm + broadcast, column-parallel
  * gate/up + SwiGLU, row-parallel ff_out pushed, reduce + residual + next norm (ln_f after the last layer) + broadcast.
- * On return (stream order) every rank's xn buffer holds ln_f(x) for all B*L rows. Pointers are device pointers owned by the caller. */
+ * On return (stream order) every rank's xn buffer holds ln_f(x) for all B*L rows. Pointers are device pointers owned by the caller.
+ * Grouped-query shards: d_kv = 128 * n_kv_heads_local (the kv heads this rank's query heads read; local query head j reads local
+ * kv head j / (n_heads_local / n_kv_heads_local)). A layer of such a shard, or one with a q/k/v bias, runs the grouped-query QKV
+ * epilogue (mmdp_qkv_rope_tp_gqa) and the grouped-query attention; the multi-head shard without a bias runs mmdp_qkv_rope_tp's. */
 typedef struct mmdp_tp_layer {
-    const uint16_t* wqkv;       /* [3 * d_attn, d]  q | k | v rows of the local heads */
+    const uint16_t* wqkv;       /* [d_attn + 2 * d_kv, d]  q rows of the local heads | k rows of the local kv heads | v rows of the same */
     const uint16_t* wo;         /* [d, d_attn] */
     const uint16_t* w13;        /* [2 * ff_local, d] gate / up interleaved in 128-row blocks */
     const uint16_t* w2;         /* [d, ff_local] */
     const uint16_t* attn_norm;  /* [d] */
     const uint16_t* ff_norm;    /* [d] */
+    const uint16_t* bqkv;       /* [d_attn + 2 * d_kv] the matching slices of q_proj | k_proj | v_proj's bias, or NULL (no bias) */
 } mmdp_tp_layer;
 /* Shared (peer-mapped) state of one ROW CHUNK of the tensor-parallel forward. The sequence rows are cut into n_chunks (1 or 2)
  * contiguous chunks; inside a chunk rank r owns rows [r*R, (r+1)*R), R = ceil(rows of the chunk / n_ranks). With two chunks
@@ -121,11 +125,13 @@ typedef struct mmdp_tp_ctx {
     const mmdp_tp_layer* layers;                 /* HOST array [n_layers] */
     const uint16_t* wte; const uint16_t* ln_f; int64_t vocab;
     const float* cos_tab; const float* sin_tab;  /* [max_seq_len, 64] */
-    uint16_t *q, *k, *att, *h, *vt;              /* work buffers: [M, d_attn] x3, [M, ff_local], [B, H_local, 128, Lpad] (pad columns zero) */
+    uint16_t *q, *k, *att, *h, *vt;              /* work buffers: q, att [M, d_attn], k [M, d_kv], h [M, ff_local],
+                                                    vt [B, n_kv_heads_local, 128, Lpad] (pad columns zero) */
     uint16_t* const* xn;                         /* HOST array [n_ranks] of the activation buffers [M, d] */
     int32_t n_chunks;                            /* 1 or 2 */
     int32_t chunk_rows0;                         /* rows of chunk 0 (chunk 1 holds the rest); ignored when n_chunks == 1 */
     mmdp_tp_chunk chunk[2];
+    int32_t n_kv_heads_local;                    /* kv heads of the shard, dividing n_heads_local; 0 = n_heads_local (multi-head) */
 } mmdp_tp_ctx;
 /* epoch0: the last epoch used so far; the call uses epoch0 + 1 ... epoch0 + 2 * n_layers + 1 on every chunk's flags (returned
  * through *epoch_out). With two chunks the call uses an internal second stream, forked from and joined back into `stream`. */
@@ -180,6 +186,14 @@ MMDP_API int mmdp_qkv_rope_tp(const uint16_t* A, int lda, const uint16_t* Wqkv, 
 MMDP_API int mmdp_qkv_rope_gqa(const uint16_t* A, int lda, const uint16_t* Wqkv, const uint16_t* bias, int M, int d_model, int n_heads,
                                int n_kv_heads, int L, int Lpad, const float* cos_tab, const float* sin_tab, uint16_t* q, uint16_t* k,
                                uint16_t* vt, void* stream);
+
+/* Tensor-parallel shard of the grouped-query projection: Wqkv = [q rows of this rank's n_heads_local heads | k rows of its
+ * n_kv_heads_local kv heads | v rows of the same] ([128 * (n_heads_local + 2 * n_kv_heads_local), d_model]); bias (nullable) the
+ * matching slices of the q / k / v biases. K = d_model; q [B*L, 128*n_heads_local], k [B*L, 128*n_kv_heads_local], vt [B,
+ * n_kv_heads_local, 128, Lpad]. n_kv_heads_local divides n_heads_local. */
+MMDP_API int mmdp_qkv_rope_tp_gqa(const uint16_t* A, int lda, const uint16_t* Wqkv, const uint16_t* bias, int M, int d_model,
+                                  int n_heads_local, int n_kv_heads_local, int L, int Lpad, const float* cos_tab, const float* sin_tab,
+                                  uint16_t* q, uint16_t* k, uint16_t* vt, void* stream);
 
 /* x = bf16(bf16(partial) + x): residual add of an fp32 partial-sum buffer that was all-reduced across tensor-parallel ranks
  * (keeps the reference's rounding points: nn.Linear output -> bf16, then the residual add -> bf16). */

@@ -52,7 +52,7 @@ class VqModelConfig(C.Structure):
 
 
 class TpLayer(C.Structure):
-    _fields_ = [(n, C.c_void_p) for n in ("wqkv", "wo", "w13", "w2", "attn_norm", "ff_norm")]
+    _fields_ = [(n, C.c_void_p) for n in ("wqkv", "wo", "w13", "w2", "attn_norm", "ff_norm", "bqkv")]
 
 
 class TpChunk(C.Structure):
@@ -64,7 +64,8 @@ class TpCtx(C.Structure):
                 ("n_ranks", C.c_int32), ("rank", C.c_int32), ("rms_eps", C.c_float), ("layers", C.POINTER(TpLayer)),
                 ("wte", C.c_void_p), ("ln_f", C.c_void_p), ("vocab", C.c_int64), ("cos_tab", C.c_void_p), ("sin_tab", C.c_void_p),
                 ("q", C.c_void_p), ("k", C.c_void_p), ("att", C.c_void_p), ("h", C.c_void_p), ("vt", C.c_void_p),
-                ("xn", C.POINTER(C.c_void_p)), ("n_chunks", C.c_int32), ("chunk_rows0", C.c_int32), ("chunk", TpChunk * 2)]
+                ("xn", C.POINTER(C.c_void_p)), ("n_chunks", C.c_int32), ("chunk_rows0", C.c_int32), ("chunk", TpChunk * 2),
+                ("n_kv_heads_local", C.c_int32)]
 
 
 class ModelConfig(C.Structure):
@@ -105,6 +106,7 @@ SIGNATURES = {
     "mmdp_qkv_rope": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mmdp_qkv_rope_tp": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mmdp_qkv_rope_gqa": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "mmdp_qkv_rope_tp_gqa": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mmdp_resid_add_f32": (_i, [_vp, _i, _vp, _i, _i, _i, _vp]),
     "mmdp_attention": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp]),
     "mmdp_attention_packed": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _f, _vp]),

@@ -215,6 +215,17 @@ MMDP_API int mmdp_qkv_rope_tp(const uint16_t* A, int lda, const uint16_t* Wqkv, 
                      &qa, (cudaStream_t)stream);
 }
 
+MMDP_API int mmdp_qkv_rope_tp_gqa(const uint16_t* A, int lda, const uint16_t* Wqkv, const uint16_t* bias, int M, int d_model,
+                                  int n_heads_local, int n_kv_heads_local, int L, int Lpad, const float* cos_tab, const float* sin_tab,
+                                  uint16_t* q, uint16_t* k, uint16_t* vt, void* stream) {
+    const int d_attn = n_heads_local * 128;
+    QkvRopeArgs qa{(bf16*)q, (bf16*)k, (bf16*)vt, cos_tab, sin_tab, L, Lpad, d_attn, n_heads_local};
+    qa.n_kv_heads = n_kv_heads_local;
+    qa.bias = (const bf16*)bias;
+    return gemm_bf16(EPI_QKVGQA, (const bf16*)A, lda, (const bf16*)Wqkv, d_model, M, d_attn + 2 * 128 * n_kv_heads_local, d_model,
+                     nullptr, 0, nullptr, 0, &qa, (cudaStream_t)stream);
+}
+
 MMDP_API int mmdp_resid_add_f32(uint16_t* x, int ldx, const float* partial, int ldp, int M, int d, void* stream) {
     return resid_add_f32((bf16*)x, ldx, partial, ldp, M, d, (cudaStream_t)stream);
 }
@@ -385,6 +396,10 @@ MMDP_API int mmdp_tp_forward(const mmdp_tp_ctx* c, const int64_t* ids, int B, in
     if (!c || !ids || !epoch_out) return set_error("mmdp_tp_forward: null argument");
     cudaStream_t s0 = (cudaStream_t)stream;
     const int d = c->d_model, Hl = c->n_heads_local, da = Hl * 128, ffl = c->ff_local, tp = c->n_ranks;
+    // kv heads of this rank's shard: 0 = Hl (the multi-head shard)
+    const int Hkv = c->n_kv_heads_local ? c->n_kv_heads_local : Hl, dkv = Hkv * 128;
+    if (Hkv <= 0 || Hkv > Hl || Hl % Hkv)
+        return set_error("mmdp_tp_forward: n_kv_heads_local=%d must divide n_heads_local=%d", c->n_kv_heads_local, Hl);
     const int M = B * L, Lpad = ((L + 7) / 8) * 8;
     const int nch = c->n_chunks == 2 ? 2 : 1;
     if (nch == 2 && (c->chunk_rows0 <= 0 || c->chunk_rows0 >= M)) return set_error("mmdp_tp_forward: chunk_rows0 must lie inside (0, %d)", M);
@@ -443,15 +458,25 @@ MMDP_API int mmdp_tp_forward(const mmdp_tp_ctx* c, const int64_t* ids, int B, in
     }
     for (int li = 0; li < c->n_layers; ++li) {
         const mmdp_tp_layer& l = c->layers[li];
+        // a grouped-query or biased shard runs the grouped-query epilogue; the multi-head shard keeps EPI_QKVROPE
+        const bool gqa = Hkv != Hl || l.bqkv;
         for (int ci = 0; ci < nch; ++ci) {
             const Chunk& k = ch[ci];
+            if (gqa) {
+                QkvRopeArgs qa{(bf16*)c->q + (size_t)k.m0 * da, (bf16*)c->k + (size_t)k.m0 * dkv, (bf16*)c->vt, c->cos_tab, c->sin_tab, L, Lpad, da, Hl};
+                qa.chunked = nch > 1; qa.row0 = k.m0;
+                qa.n_kv_heads = Hkv; qa.bias = (const bf16*)l.bqkv;
+                if (gemm_bf16(EPI_QKVGQA, xn + (size_t)k.m0 * d, d, (const bf16*)l.wqkv, d, k.Mc, da + 2 * dkv, d, nullptr, 0, nullptr, 0, &qa, k.s))
+                    return -1;
+                continue;
+            }
             QkvRopeArgs qa{(bf16*)c->q + (size_t)k.m0 * da, (bf16*)c->k + (size_t)k.m0 * da, (bf16*)c->vt, c->cos_tab, c->sin_tab, L, Lpad, da, Hl};
             qa.chunked = nch > 1; qa.row0 = k.m0;
             if (gemm_bf16(EPI_QKVROPE, xn + (size_t)k.m0 * d, d, (const bf16*)l.wqkv, d, k.Mc, 3 * da, d, nullptr, 0, nullptr, 0, &qa, k.s)) return -1;
         }
         // attention mixes all rows: both chunks' q / k / v^T must be complete, and it must be complete before either chain goes on
         if (join()) return -1;
-        if (attention_fwd((const bf16*)c->q, (const bf16*)c->k, (const bf16*)c->vt, (bf16*)c->att, B, Hl, L, Lpad, scale, s0)) return -1;
+        if (attention_fwd((const bf16*)c->q, (const bf16*)c->k, (const bf16*)c->vt, (bf16*)c->att, B, Hl, L, Lpad, scale, s0, 0, Hkv)) return -1;
         if (fork()) return -1;
         const uint32_t e1 = ++epoch, e2 = ++epoch;
         for (int ci = 0; ci < nch; ++ci) {

@@ -51,17 +51,19 @@ struct GemmParams {
     const __nv_bfloat16* bias;
 };
 
-// Host-side argument check of the grouped-query QKV epilogues (bf16 and e4m3 GEMM). The token-cache and row-chunked
-// launches stay on the multi-head epilogue.
+// Host-side argument check of the grouped-query QKV epilogues (bf16 and e4m3 GEMM). The token-cache launch stays on the
+// multi-head epilogue; a row-chunked launch (the tensor-parallel forward's second chunk) takes positions and V^T through row0
+// as EPI_QKVROPE does (qkv_row_coords), q / k relative to the chunk.
 inline int qkv_gqa_check(const char* who, int epi, int M, int N, const QkvRopeArgs* qa) {
     if (!qa) return set_error("%s: qkv epilogue needs QkvRopeArgs", who);
     const int d = qa->d_model, H = qa->n_heads, Hkv = qa->n_kv_heads;
     if (d % 256 || d != H * 128) return set_error("%s: qkv epilogue needs head_dim 128 and d_model %% 256 == 0", who);
     if (Hkv <= 0 || Hkv > H || H % Hkv) return set_error("%s: n_kv_heads=%d must divide n_heads=%d", who, Hkv, H);
     if (N != d + 2 * 128 * Hkv) return set_error("%s: grouped-query qkv needs N == d_model + 2 * 128 * n_kv_heads", who);
-    if (qa->pos_map || qa->chunked || qa->row0) return set_error("%s: grouped-query qkv has no token-cache or row-chunked form", who);
-    if (epi == EPI_QKVGQA_PACKED ? !qa->seg_pos : (qa->L <= 0 || M % qa->L))
-        return set_error("%s: qkv epilogue needs M == B*L (or a packed row map)", who);
+    if (qa->pos_map) return set_error("%s: grouped-query qkv has no token-cache form", who);
+    if (qa->row0 < 0) return set_error("%s: row0 must not be negative", who);
+    if (epi == EPI_QKVGQA_PACKED ? (!qa->seg_pos || qa->chunked || qa->row0) : (qa->L <= 0 || (!qa->chunked && M % qa->L)))
+        return set_error("%s: qkv epilogue needs M == B*L (or a row chunk of it, or a packed row map)", who);
     return 0;
 }
 

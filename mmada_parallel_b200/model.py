@@ -62,8 +62,7 @@ def effective_n_kv_heads(config, n_heads: int) -> int:
 def check_supported_config(config, n_heads: int, grouped_query: bool = False) -> int:
     """Features of the reference config this path does not implement must fail loudly, not silently differ (shared by the
     single-GPU and the tensor-parallel model). Returns the number of kv heads. grouped_query: the caller runs
-    n_kv_heads < n_heads and include_qkv_bias (the single-GPU model); the tensor-parallel model, which can only be
-    checked on several GPUs, refuses both."""
+    n_kv_heads < n_heads and include_qkv_bias (both models pass True); without it both are refused."""
     g = lambda k, dflt=None: getattr(config, k, dflt)
     n_kv = effective_n_kv_heads(config, n_heads)
     if not grouped_query and n_kv != n_heads:

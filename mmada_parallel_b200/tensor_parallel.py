@@ -1,7 +1,8 @@
 """Tensor-parallel forward for the single-sample case (BASELINE config 4): one sample's transformer forward split over the
 GPUs of one node. The reference has no tensor parallelism (SURVEY.md 2c); this follows SURVEY.md 8e:
 
-  * attention: heads split (q/k/v_proj column-parallel, attn_out row-parallel); MLP: ff split (ff_proj/up_proj
+  * attention: heads split (q/k/v_proj column-parallel, attn_out row-parallel; with grouped-query or multi-query attention each
+    rank computes the kv heads its query heads read, see kv_shard); MLP: ff split (ff_proj/up_proj
     column-parallel, ff_out row-parallel); LM head: vocabulary rows split (and the VQ-codebook window split separately);
   * the two row-parallel GEMMs per layer produce fp32 PARTIAL sums (MMDP_EPI_F32). What follows them - the cross-rank sum,
     the residual add, the NEXT RMSNorm and the distribution of its output to all ranks - is one kernel per rank over NVLink
@@ -33,10 +34,27 @@ from ._lib import EPI_F32, EPI_PLAIN, EPI_SWIGLU, check, lib, ptr, stream_ptr
 from .model import ModelOutput, check_supported_config, rope_tables
 
 
+def kv_shard(n_heads: int, n_kv_heads: int, rank: int, tp: int):
+    """The kv heads rank `rank` of `tp` computes: (first kv head, count). Rank r owns query heads [r H / tp, (r + 1) H / tp), and
+    query head h reads kv head h // (H / Hkv).
+      * tp divides Hkv: rank r owns kv heads [r Hkv / tp, (r + 1) Hkv / tp), exactly those its query heads read;
+      * Hkv divides tp (multi-query attention included): rank r computes the one kv head r Hkv // tp that all its query heads
+        read; that kv head is computed on tp / Hkv ranks.
+    Any other (tp, Hkv) pair would split one rank's query heads over kv heads owned by different ranks: ValueError."""
+    if n_kv_heads % tp == 0:
+        return rank * (n_kv_heads // tp), n_kv_heads // tp
+    if tp % n_kv_heads == 0:
+        return rank * n_kv_heads // tp, 1
+    raise ValueError(f"tp={tp} and n_kv_heads={n_kv_heads}: one of the two must divide the other (each rank computes whole kv heads "
+                     "for its query heads)")
+
+
 def shard_state_dict(sd: Dict[str, torch.Tensor], n_layers: int, n_heads: int, rank: int, tp: int, vq_col0: int,
-                     vq_cols: int) -> Dict[str, torch.Tensor]:
+                     vq_cols: int, *, n_kv_heads: Optional[int] = None, qkv_bias: bool = False) -> Dict[str, torch.Tensor]:
     """Slices a full HF state dict (names of SURVEY.md 8b) into rank `rank`'s tensor-parallel shard. Pure tensor slicing
-    (device agnostic) so it is unit-tested on the CPU."""
+    (device agnostic) so it is unit-tested on the CPU. n_kv_heads (None: n_heads) and the kv heads of the shard follow kv_shard;
+    `blocks.i.wqkv` holds the q rows of the local heads, then the k rows and the v rows of the local kv heads, and with qkv_bias
+    `blocks.i.bqkv` the matching slices of the q / k / v biases."""
     g = lambda n: sd["model.transformer." + n] if ("model.transformer." + n) in sd else sd[n]
     out = {"wte": g("wte.weight"), "ln_f": g("ln_f.weight")}
     head = g("ff_out.weight")
@@ -44,13 +62,17 @@ def shard_state_dict(sd: Dict[str, torch.Tensor], n_layers: int, n_heads: int, r
     if n_heads % tp or V % tp or vq_cols % tp:
         raise ValueError(f"tp={tp} must divide n_heads={n_heads}, vocab rows={V} and the codebook window={vq_cols}")
     da = (n_heads // tp) * 128
+    kv0, n_kv_local = kv_shard(n_heads, n_kv_heads or n_heads, rank, tp)
+    kv = slice(kv0 * 128, (kv0 + n_kv_local) * 128)
     out["head"] = head[rank * (V // tp):(rank + 1) * (V // tp)]
     c = vq_cols // tp
     out["head_vq"] = head[vq_col0 + rank * c: vq_col0 + (rank + 1) * c]
     for i in range(n_layers):
         p = f"blocks.{i}."
         sl = slice(rank * da, (rank + 1) * da)
-        out[p + "wqkv"] = torch.cat([g(p + "q_proj.weight")[sl], g(p + "k_proj.weight")[sl], g(p + "v_proj.weight")[sl]], dim=0)
+        out[p + "wqkv"] = torch.cat([g(p + "q_proj.weight")[sl], g(p + "k_proj.weight")[kv], g(p + "v_proj.weight")[kv]], dim=0)
+        if qkv_bias:
+            out[p + "bqkv"] = torch.cat([g(p + "q_proj.bias")[sl], g(p + "k_proj.bias")[kv], g(p + "v_proj.bias")[kv]], dim=0)
         out[p + "wo"] = g(p + "attn_out.weight")[:, sl]
         ffp, up = g(p + "ff_proj.weight"), g(p + "up_proj.weight")
         ff = ffp.shape[0]
@@ -159,25 +181,30 @@ class TensorParallelLLaDA:
         self.ff = int(g("mlp_hidden_size") or g("mlp_ratio", 4) * self.d_model)
         self.vocab_rows = int(g("embedding_size") or g("vocab_size"))
         self.rms_eps = float(g("rms_norm_eps", 1e-5))
-        check_supported_config(config, self.n_heads)
+        self.n_kv_heads = check_supported_config(config, self.n_heads, grouped_query=True)
+        self.qkv_bias = bool(g("include_qkv_bias", False))
         self.h_local = self.n_heads // tp_size
         self.d_attn = self.h_local * 128
         if self.d_attn % 256:
             raise ValueError("n_heads / tp must be even (the fused QKV+RoPE epilogue works on 2-head tiles)")
+        self.kv_local = kv_shard(self.n_heads, self.n_kv_heads, tp_rank, tp_size)[1]
+        # a grouped-query or biased shard runs the grouped-query QKV epilogue and attention; the multi-head shard keeps its kernels
+        self.gqa = self.kv_local != self.h_local or self.qkv_bias
         self.ff_local = self.ff // tp_size
         self.v_local = self.vocab_rows // tp_size
         self.vq_col0, self.vq_cols = text_vocab_size, codebook_size
         self.c_local = codebook_size // tp_size
         self.max_seq_len = int(max_seq_len or g("max_sequence_length", 4096))
         self.max_batch = max_batch
-        sh = shard_state_dict(state_dict, self.n_layers, self.n_heads, tp_rank, tp_size, text_vocab_size, codebook_size)
+        sh = shard_state_dict(state_dict, self.n_layers, self.n_heads, tp_rank, tp_size, text_vocab_size, codebook_size,
+                              n_kv_heads=self.n_kv_heads, qkv_bias=self.qkv_bias)
         self.w = {k: v.detach().to(device=self.device, dtype=torch.bfloat16).contiguous() for k, v in sh.items()}
         cos, sin = rope_tables(128, float(g("rope_theta", 10000.0)), self.max_seq_len)
         self.cos, self.sin = cos.to(self.device), sin.to(self.device)
         M, d, bf = self.max_batch * self.max_seq_len, self.d_model, dict(dtype=torch.bfloat16, device=self.device)
         self.Mmax = M
         self.q = torch.empty((M, self.d_attn), **bf)
-        self.k = torch.empty((M, self.d_attn), **bf)
+        self.k = torch.empty((M, self.kv_local * 128), **bf)
         self.att = torch.empty((M, self.d_attn), **bf)
         self.h = torch.empty((M, self.ff_local), **bf)
         self.vt = None
@@ -245,9 +272,15 @@ class TensorParallelLLaDA:
         for i in range(self.n_layers):
             p = f"blocks.{i}."
             check(lib.mmdp_rmsnorm(ptr(x), d, None, ptr(w[p + "attn_norm"]), ptr(xn), d, M, d, self.rms_eps, s))
-            check(lib.mmdp_qkv_rope_tp(ptr(xn), d, ptr(w[p + "wqkv"]), M, d, self.h_local, L, Lpad, ptr(self.cos), ptr(self.sin),
-                                       ptr(self.q), ptr(self.k), ptr(self.vt), s))
-            check(lib.mmdp_attention(ptr(self.q), ptr(self.k), ptr(self.vt), ptr(self.att), B, self.h_local, L, Lpad, scale, s))
+            if self.gqa:
+                check(lib.mmdp_qkv_rope_tp_gqa(ptr(xn), d, ptr(w[p + "wqkv"]), ptr(w.get(p + "bqkv")), M, d, self.h_local, self.kv_local,
+                                               L, Lpad, ptr(self.cos), ptr(self.sin), ptr(self.q), ptr(self.k), ptr(self.vt), s))
+                check(lib.mmdp_attention_gqa(ptr(self.q), ptr(self.k), ptr(self.vt), ptr(self.att), B, None, self.h_local, self.kv_local,
+                                             L, Lpad, scale, s))
+            else:
+                check(lib.mmdp_qkv_rope_tp(ptr(xn), d, ptr(w[p + "wqkv"]), M, d, self.h_local, L, Lpad, ptr(self.cos), ptr(self.sin),
+                                           ptr(self.q), ptr(self.k), ptr(self.vt), s))
+                check(lib.mmdp_attention(ptr(self.q), ptr(self.k), ptr(self.vt), ptr(self.att), B, self.h_local, L, Lpad, scale, s))
             check(lib.mmdp_gemm_bf16(EPI_F32, ptr(self.att), self.d_attn, ptr(w[p + "wo"]), self.d_attn, M, d, self.d_attn,
                                      ptr(self.part), d, None, 0, s))
             self._allreduce(self.part[:M])
@@ -272,8 +305,11 @@ class TensorParallelLLaDA:
             for name, t in (("wqkv", w[p + "wqkv"]), ("wo", w[p + "wo"]), ("w13", w[p + "w13"]), ("w2", w[p + "w2"]),
                             ("attn_norm", w[p + "attn_norm"]), ("ff_norm", w[p + "ff_norm"])):
                 setattr(layers[i], name, t.data_ptr())
+            if self.qkv_bias:
+                layers[i].bqkv = w[p + "bqkv"].data_ptr()
         c = _lib.TpCtx()
         c.d_model, c.n_heads_local, c.ff_local, c.n_layers, c.n_ranks, c.rank = self.d_model, self.h_local, self.ff_local, self.n_layers, self.tp, self.rank
+        c.n_kv_heads_local = self.kv_local
         c.rms_eps = self.rms_eps
         c.layers = layers
         c.wte, c.ln_f, c.vocab = w["wte"].data_ptr(), w["ln_f"].data_ptr(), w["wte"].shape[0]
@@ -301,7 +337,7 @@ class TensorParallelLLaDA:
             raise _lib.MmdpError("TensorParallelLLaDA: batch x length exceeds the workspace")
         Lpad = (L + 7) // 8 * 8
         if self._vt_key != (B, Lpad, L):
-            self.vt = torch.zeros((B, self.h_local, 128, Lpad), dtype=torch.bfloat16, device=self.device)
+            self.vt = torch.zeros((B, self.kv_local, 128, Lpad), dtype=torch.bfloat16, device=self.device)
             self._vt_key = (B, Lpad, L)
         wte = self.w["wte"]
         if self.collective == "p2p":
