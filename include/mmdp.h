@@ -92,6 +92,23 @@ MMDP_API int mmdp_tp_reduce_norm(const float* recv_local, int rows_per_rank, int
                         int n_ranks, int my_rank, uint16_t* x_shard, const uint16_t* weight, int row0, int nrows, int d, float eps,
                         uint32_t epoch, uint32_t* done_counter, void* stream);
 
+/* FP8 (e4m3) forms of the two collective kernels, for a tensor-parallel model whose block linears run in FP8:
+ *   mmdp_gemm_fp8_f32                 C [M, ldc] fp32 = sw[n] * sum_g sa[g][m] * sum_{k in g} A[m,k] W[n,k] (mmdp_gemm_fp8's
+ *                                     arithmetic without the bf16 rounding): the partial sum of a row-parallel FP8 linear
+ *   mmdp_gemm_fp8_f32_scatter         the same rows PUSHED to their owners, in mmdp_gemm_f32_scatter's layout and with its checks
+ *   mmdp_tp_reduce_norm_fp8           mmdp_tp_reduce_norm whose broadcast carries e4m3 instead of bf16: every normalised row it
+ *                                     owns goes to every rank as e4m3 bytes xq[r] + row * d and 1 x 128 group scales
+ *                                     xs[r][g * ld_s + row] (ld_s >= row0 + nrows; d % 128 == 0). Bytes and scales are bitwise
+ *                                     mmdp_quantize_fp8(group = 128) of the bf16 rows mmdp_tp_reduce_norm would have stored:
+ *                                     d + d/32 bytes per row and rank instead of 2d, and no rank quantises the activations again. */
+MMDP_API int mmdp_gemm_fp8_f32(const uint8_t* A, int lda, const float* sa, const uint8_t* W, int ldw, const float* sw, int M, int N, int K,
+                               float* C, int ldc, void* stream);
+MMDP_API int mmdp_gemm_fp8_f32_scatter(const uint8_t* A, int lda, const float* sa, const uint8_t* W, int ldw, const float* sw, int M, int N,
+                                       int K, float* const* recv, int n_ranks, int rows_per_rank, int slot, void* stream);
+MMDP_API int mmdp_tp_reduce_norm_fp8(const float* recv_local, int rows_per_rank, int n_src, uint8_t* const* xq, float* const* xs, int ld_s,
+                                     uint32_t* const* flags, int n_ranks, int my_rank, uint16_t* x_shard, const uint16_t* weight, int row0,
+                                     int nrows, int d, float eps, uint32_t epoch, uint32_t* done_counter, void* stream);
+
 /* The whole tensor-parallel body in one call (the per-layer sequence TensorParallelLLaDA used to issue from Python: ~10 launches
  * per layer left a TP=8 rank CPU-bound): embedding of this rank's rows, norm + broadcast, then per layer column-parallel QKV+RoPE,
  * attention on the local heads, row-parallel attn_out pushed to the owners, reduce + residual + ff_norm + broadcast, column-parallel
@@ -109,6 +126,16 @@ typedef struct mmdp_tp_layer {
     const uint16_t* ff_norm;    /* [d] */
     const uint16_t* bqkv;       /* [d_attn + 2 * d_kv] the matching slices of q_proj | k_proj | v_proj's bias, or NULL (no bias) */
 } mmdp_tp_layer;
+/* FP8 shard of a layer's four linears (mmdp_tp_ctx.precision == MMDP_PRECISION_FP8): every weight quantised WHOLE as in an FP8
+ * context (one scale per row over the full K), then sliced: the column-parallel linears keep their rows and row scales, the
+ * row-parallel ones (wo, w2) their K-columns of the e4m3 bytes and the full row scales [d]. */
+typedef struct mmdp_tp_layer_fp8 {
+    const uint8_t* wqkv;        /* [d_attn + 2 * d_kv, d] e4m3, rows as mmdp_tp_layer.wqkv */
+    const uint8_t* wo;          /* [d, d_attn] */
+    const uint8_t* w13;         /* [2 * ff_local, d] gate / up interleaved in 64-row blocks (the FP8 tile is 128 wide) */
+    const uint8_t* w2;          /* [d, ff_local] */
+    const float *sqkv, *so, *s13, *s2;  /* row scales: [d_attn + 2 * d_kv], [d], [2 * ff_local] (interleaved as w13), [d] */
+} mmdp_tp_layer_fp8;
 /* Shared (peer-mapped) state of one ROW CHUNK of the tensor-parallel forward. The sequence rows are cut into n_chunks (1 or 2)
  * contiguous chunks; inside a chunk rank r owns rows [r*R, (r+1)*R), R = ceil(rows of the chunk / n_ranks). With two chunks
  * the attn_out / MLP part of a layer runs as two independent chains on two streams, so that one chunk's NVLink traffic
@@ -132,6 +159,17 @@ typedef struct mmdp_tp_ctx {
     int32_t chunk_rows0;                         /* rows of chunk 0 (chunk 1 holds the rest); ignored when n_chunks == 1 */
     mmdp_tp_chunk chunk[2];
     int32_t n_kv_heads_local;                    /* kv heads of the shard, dividing n_heads_local; 0 = n_heads_local (multi-head) */
+    /* precision of the four block linears: MMDP_PRECISION_BF16 (0) or MMDP_PRECISION_FP8. In FP8 the layers' bf16 linear pointers
+     * are unused (norms and bias still come from `layers`); every reduce but the last broadcasts e4m3 rows (mmdp_tp_reduce_norm_fp8)
+     * that the QKV and gate/up GEMMs read, att and h are quantised locally before attn_out / ff_out, and the last reduce (ln_f)
+     * stays bf16 into xn. */
+    int32_t precision;
+    const mmdp_tp_layer_fp8* layers_fp8;         /* FP8: HOST array [n_layers] */
+    uint8_t* const* xq;                          /* FP8: HOST array [n_ranks] of the e4m3 activation buffers [M, d] */
+    float* const* xq_scales;                     /* FP8: HOST array [n_ranks] of their scales, M * d / 128 fp32: row chunk c (rows
+                                                    [m0, m0 + Mc)) at offset m0 * d / 128, laid out [d / 128][Mc] */
+    uint8_t* a8;                                 /* FP8: local e4m3 copy of att / h, M * max(d_attn, ff_local) bytes */
+    float* a8_scales;                            /* FP8: its scales, M * max(d_attn, ff_local) / 128 fp32 */
 } mmdp_tp_ctx;
 /* epoch0: the last epoch used so far; the call uses epoch0 + 1 ... epoch0 + 2 * n_layers + 1 on every chunk's flags (returned
  * through *epoch_out). With two chunks the call uses an internal second stream, forked from and joined back into `stream`. */
@@ -194,6 +232,14 @@ MMDP_API int mmdp_qkv_rope_gqa(const uint16_t* A, int lda, const uint16_t* Wqkv,
 MMDP_API int mmdp_qkv_rope_tp_gqa(const uint16_t* A, int lda, const uint16_t* Wqkv, const uint16_t* bias, int M, int d_model,
                                   int n_heads_local, int n_kv_heads_local, int L, int Lpad, const float* cos_tab, const float* sin_tab,
                                   uint16_t* q, uint16_t* k, uint16_t* vt, void* stream);
+
+/* FP8 form of the tensor-parallel shard's projection (mmdp_qkv_rope_tp / _gqa with e4m3 operands, mmdp_gemm_fp8's arithmetic):
+ * A e4m3 [M, d_model] with scales sa [d_model / 128][M], Wqkv e4m3 [128 * (n_heads_local + 2 * n_kv_heads_local), d_model] with
+ * row scales sw. A multi-head shard without a bias (n_kv_heads_local == n_heads_local, bias NULL) runs mmdp_qkv_rope_tp's
+ * epilogue, any other the grouped-query one, as mmdp_tp_forward does. Outputs as mmdp_qkv_rope_tp_gqa. */
+MMDP_API int mmdp_qkv_rope_tp_fp8(const uint8_t* A, int lda, const float* sa, const uint8_t* Wqkv, const float* sw, const uint16_t* bias,
+                                  int M, int d_model, int n_heads_local, int n_kv_heads_local, int L, int Lpad, const float* cos_tab,
+                                  const float* sin_tab, uint16_t* q, uint16_t* k, uint16_t* vt, void* stream);
 
 /* x = bf16(bf16(partial) + x): residual add of an fp32 partial-sum buffer that was all-reduced across tensor-parallel ranks
  * (keeps the reference's rounding points: nn.Linear output -> bf16, then the residual add -> bf16). */

@@ -55,6 +55,10 @@ class TpLayer(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("wqkv", "wo", "w13", "w2", "attn_norm", "ff_norm", "bqkv")]
 
 
+class TpLayerFp8(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("wqkv", "wo", "w13", "w2", "sqkv", "so", "s13", "s2")]
+
+
 class TpChunk(C.Structure):
     _fields_ = [("x_shard", C.c_void_p), ("recv", C.POINTER(C.c_void_p) * 2), ("flags", C.POINTER(C.c_void_p)), ("done_counter", C.c_void_p)]
 
@@ -65,7 +69,8 @@ class TpCtx(C.Structure):
                 ("wte", C.c_void_p), ("ln_f", C.c_void_p), ("vocab", C.c_int64), ("cos_tab", C.c_void_p), ("sin_tab", C.c_void_p),
                 ("q", C.c_void_p), ("k", C.c_void_p), ("att", C.c_void_p), ("h", C.c_void_p), ("vt", C.c_void_p),
                 ("xn", C.POINTER(C.c_void_p)), ("n_chunks", C.c_int32), ("chunk_rows0", C.c_int32), ("chunk", TpChunk * 2),
-                ("n_kv_heads_local", C.c_int32)]
+                ("n_kv_heads_local", C.c_int32), ("precision", C.c_int32), ("layers_fp8", C.POINTER(TpLayerFp8)),
+                ("xq", C.POINTER(C.c_void_p)), ("xq_scales", C.POINTER(C.c_void_p)), ("a8", C.c_void_p), ("a8_scales", C.c_void_p)]
 
 
 class ModelConfig(C.Structure):
@@ -100,6 +105,9 @@ SIGNATURES = {
     "mmdp_tp_forward": (_i, [C.POINTER(TpCtx), _vp, _i, _i, C.c_uint32, C.POINTER(C.c_uint32), _vp]),
     "mmdp_gemm_f32_scatter": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),
     "mmdp_tp_reduce_norm": (_i, [_vp, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _i, _f, C.c_uint32, _vp, _vp]),
+    "mmdp_gemm_fp8_f32": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _i, _i, _vp, _i, _vp]),
+    "mmdp_gemm_fp8_f32_scatter": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _i, _i, _vp, _i, _i, _i, _vp]),
+    "mmdp_tp_reduce_norm_fp8": (_i, [_vp, _i, _i, _vp, _vp, _i, _vp, _i, _i, _vp, _vp, _i, _i, _i, _f, C.c_uint32, _vp, _vp]),
     "mmdp_gemm_bf16": (_i, [_i, _vp, _i, _vp, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp]),
     "mmdp_quantize_fp8": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _vp, _vp]),
     "mmdp_gemm_fp8": (_i, [_i, _vp, _i, _vp, _vp, _i, _vp, _i, _i, _i, _vp, _i, _vp, _i, _vp]),
@@ -107,6 +115,7 @@ SIGNATURES = {
     "mmdp_qkv_rope_tp": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mmdp_qkv_rope_gqa": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mmdp_qkv_rope_tp_gqa": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "mmdp_qkv_rope_tp_fp8": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mmdp_resid_add_f32": (_i, [_vp, _i, _vp, _i, _i, _i, _vp]),
     "mmdp_attention": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp]),
     "mmdp_attention_packed": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _f, _vp]),

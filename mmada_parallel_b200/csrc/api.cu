@@ -226,6 +226,19 @@ MMDP_API int mmdp_qkv_rope_tp_gqa(const uint16_t* A, int lda, const uint16_t* Wq
                      nullptr, 0, nullptr, 0, &qa, (cudaStream_t)stream);
 }
 
+MMDP_API int mmdp_qkv_rope_tp_fp8(const uint8_t* A, int lda, const float* sa, const uint8_t* Wqkv, const float* sw, const uint16_t* bias,
+                                  int M, int d_model, int n_heads_local, int n_kv_heads_local, int L, int Lpad, const float* cos_tab,
+                                  const float* sin_tab, uint16_t* q, uint16_t* k, uint16_t* vt, void* stream) {
+    const int d_attn = n_heads_local * 128;
+    QkvRopeArgs qa{(bf16*)q, (bf16*)k, (bf16*)vt, cos_tab, sin_tab, L, Lpad, d_attn, n_heads_local};
+    if (n_kv_heads_local == n_heads_local && !bias)
+        return gemm_fp8(EPI_QKVROPE, A, lda, sa, Wqkv, d_model, sw, M, 3 * d_attn, d_model, nullptr, 0, nullptr, 0, &qa, (cudaStream_t)stream);
+    qa.n_kv_heads = n_kv_heads_local;
+    qa.bias = (const bf16*)bias;
+    return gemm_fp8(EPI_QKVGQA, A, lda, sa, Wqkv, d_model, sw, M, d_attn + 2 * 128 * n_kv_heads_local, d_model, nullptr, 0, nullptr, 0,
+                    &qa, (cudaStream_t)stream);
+}
+
 MMDP_API int mmdp_resid_add_f32(uint16_t* x, int ldx, const float* partial, int ldp, int M, int d, void* stream) {
     return resid_add_f32((bf16*)x, ldx, partial, ldp, M, d, (cudaStream_t)stream);
 }
@@ -376,6 +389,29 @@ MMDP_API int mmdp_gemm_f32_scatter(const uint16_t* A, int lda, const uint16_t* W
     return gemm_bf16(EPI_F32, (const bf16*)A, lda, (const bf16*)W, ldw, M, N, K, nullptr, N, nullptr, 0, nullptr, (cudaStream_t)stream, &sc);
 }
 
+MMDP_API int mmdp_gemm_fp8_f32(const uint8_t* A, int lda, const float* sa, const uint8_t* W, int ldw, const float* sw, int M, int N, int K,
+                               float* C, int ldc, void* stream) {
+    if (!C) return set_error("mmdp_gemm_fp8_f32: C is null");
+    return gemm_fp8(EPI_F32, A, lda, sa, W, ldw, sw, M, N, K, (bf16*)C, ldc, nullptr, 0, nullptr, (cudaStream_t)stream);
+}
+MMDP_API int mmdp_gemm_fp8_f32_scatter(const uint8_t* A, int lda, const float* sa, const uint8_t* W, int ldw, const float* sw, int M, int N,
+                                       int K, float* const* recv, int n_ranks, int rows_per_rank, int slot, void* stream) {
+    if (!recv || n_ranks < 1 || n_ranks > 8) return set_error("mmdp_gemm_fp8_f32_scatter: bad rank layout");
+    if (slot < 0 || slot >= n_ranks) return set_error("mmdp_gemm_fp8_f32_scatter: slot %d outside [0, %d)", slot, n_ranks);
+    if (rows_per_rank <= 0 || (M + rows_per_rank - 1) / rows_per_rank > n_ranks)
+        return set_error("mmdp_gemm_fp8_f32_scatter: M does not fit n_ranks x rows_per_rank");
+    GemmScatter sc{};
+    for (int r = 0; r < n_ranks; ++r) sc.dst[r] = recv[r];
+    sc.rows_per_rank = rows_per_rank; sc.slot = slot;
+    return gemm_fp8(EPI_F32, A, lda, sa, W, ldw, sw, M, N, K, nullptr, N, nullptr, 0, nullptr, (cudaStream_t)stream, &sc);
+}
+MMDP_API int mmdp_tp_reduce_norm_fp8(const float* recv_local, int rows_per_rank, int n_src, uint8_t* const* xq, float* const* xs, int ld_s,
+                                     uint32_t* const* flags, int n_ranks, int my_rank, uint16_t* x_shard, const uint16_t* weight, int row0,
+                                     int nrows, int d, float eps, uint32_t epoch, uint32_t* done_counter, void* stream) {
+    return tp_reduce_norm_fp8(recv_local, rows_per_rank, n_src, xq, xs, ld_s, flags, n_ranks, my_rank, x_shard, weight, row0, nrows, d, eps,
+                              epoch, done_counter, (cudaStream_t)stream);
+}
+
 // second stream + events of the two-chunk tensor-parallel forward, one set per device
 struct TpSide { cudaStream_t s1 = nullptr; cudaEvent_t fork = nullptr, join = nullptr; };
 static int tp_side(TpSide** out) {
@@ -402,6 +438,13 @@ MMDP_API int mmdp_tp_forward(const mmdp_tp_ctx* c, const int64_t* ids, int B, in
         return set_error("mmdp_tp_forward: n_kv_heads_local=%d must divide n_heads_local=%d", c->n_kv_heads_local, Hl);
     const int M = B * L, Lpad = ((L + 7) / 8) * 8;
     const int nch = c->n_chunks == 2 ? 2 : 1;
+    if (c->precision != MMDP_PRECISION_BF16 && c->precision != MMDP_PRECISION_FP8)
+        return set_error("mmdp_tp_forward: unknown precision %d", c->precision);
+    const bool f8 = c->precision == MMDP_PRECISION_FP8;
+    if (f8 && (!c->layers_fp8 || !c->xq || !c->xq_scales || !c->a8 || !c->a8_scales))
+        return set_error("mmdp_tp_forward: an FP8 context needs layers_fp8, xq, xq_scales, a8 and a8_scales");
+    if (f8 && (d % 128 || ffl % 128)) return set_error("mmdp_tp_forward: FP8 needs d_model and ff_local multiples of 128");
+    const int ka = da > ffl ? da : ffl;  // FP8: row stride of a chunk's region of a8 (att and h of a chunk share it)
     if (nch == 2 && (c->chunk_rows0 <= 0 || c->chunk_rows0 >= M)) return set_error("mmdp_tp_forward: chunk_rows0 must lie inside (0, %d)", M);
     // row chunks: chunk ci covers sequence rows [m0, m0 + Mc); inside it rank r owns [r * R, (r + 1) * R)
     struct Chunk { int m0, Mc, R, row0, nrows; cudaStream_t s; GemmScatter sc[2]; };
@@ -428,13 +471,32 @@ MMDP_API int mmdp_tp_forward(const mmdp_tp_ctx* c, const int64_t* ids, int B, in
     uint32_t epoch = epoch0;
     // this rank's view of every rank's activation buffer, offset to the chunk's first row
     uint16_t* xn_chunk[2][8];
+    // FP8: the same views of the e4m3 activation buffers; chunk ci's scales are a [d / 128][Mc] block at m0 * d / 128
+    uint8_t* xq_chunk[2][8];
+    float* xs_chunk[2][8];
     for (int ci = 0; ci < nch; ++ci)
-        for (int r = 0; r < tp; ++r) xn_chunk[ci][r] = c->xn[r] + (size_t)ch[ci].m0 * d;
-    auto reduce = [&](int ci, int buf, const uint16_t* w, uint32_t ep) -> int {
+        for (int r = 0; r < tp; ++r) {
+            xn_chunk[ci][r] = c->xn[r] + (size_t)ch[ci].m0 * d;
+            xq_chunk[ci][r] = f8 ? c->xq[r] + (size_t)ch[ci].m0 * d : nullptr;
+            xs_chunk[ci][r] = f8 ? c->xq_scales[r] + (size_t)ch[ci].m0 * (d / 128) : nullptr;
+        }
+    // the reduce before a column-parallel linear broadcasts e4m3 in FP8; the last one (ln_f, read by the bf16 LM head) bf16
+    auto reduce = [&](int ci, int buf, const uint16_t* w, uint32_t ep, bool to_fp8) -> int {
         const Chunk& k = ch[ci];
         const mmdp_tp_chunk& cc = c->chunk[ci];
-        return tp_reduce_norm(buf >= 0 ? cc.recv[buf][c->rank] : nullptr, k.R, buf >= 0 ? tp : 0, xn_chunk[ci], cc.flags, tp, c->rank, cc.x_shard, w,
+        const float* recv = buf >= 0 ? cc.recv[buf][c->rank] : nullptr;
+        if (to_fp8)
+            return tp_reduce_norm_fp8(recv, k.R, buf >= 0 ? tp : 0, xq_chunk[ci], xs_chunk[ci], k.Mc, cc.flags, tp, c->rank, cc.x_shard, w,
+                                      k.row0, k.nrows, d, c->rms_eps, ep, cc.done_counter, k.s);
+        return tp_reduce_norm(recv, k.R, buf >= 0 ? tp : 0, xn_chunk[ci], cc.flags, tp, c->rank, cc.x_shard, w,
                               k.row0, k.nrows, d, c->rms_eps, ep, cc.done_counter, k.s);
+    };
+    // FP8: chunk ci's local e4m3 copy of att / h (K columns) and its scales, a region of a8 no other chunk touches
+    auto quant_local = [&](int ci, const bf16* x, int K, uint8_t** q, float** sq) -> int {
+        const Chunk& k = ch[ci];
+        *q = c->a8 + (size_t)k.m0 * ka;
+        *sq = c->a8_scales + (size_t)k.m0 * (ka / 128);
+        return quantize_fp8(x, K, k.Mc, K, 128, *q, K, *sq, k.s);
     };
     auto fork = [&]() -> int {  // the side stream continues after everything issued to the caller's stream so far
         if (nch == 1) return 0;
@@ -454,25 +516,23 @@ MMDP_API int mmdp_tp_forward(const mmdp_tp_ctx* c, const int64_t* ids, int B, in
     for (int ci = 0; ci < nch; ++ci) {
         const Chunk& k = ch[ci];
         if (embed_rows(ids + k.m0 + k.row0, (const bf16*)c->wte, (bf16*)c->chunk[ci].x_shard, k.nrows, d, c->vocab, k.s, nullptr)) return -1;
-        if (reduce(ci, -1, c->layers[0].attn_norm, epoch)) return -1;
+        if (reduce(ci, -1, c->layers[0].attn_norm, epoch, f8)) return -1;
     }
     for (int li = 0; li < c->n_layers; ++li) {
         const mmdp_tp_layer& l = c->layers[li];
+        const mmdp_tp_layer_fp8* l8 = f8 ? &c->layers_fp8[li] : nullptr;
         // a grouped-query or biased shard runs the grouped-query epilogue; the multi-head shard keeps EPI_QKVROPE
         const bool gqa = Hkv != Hl || l.bqkv;
         for (int ci = 0; ci < nch; ++ci) {
             const Chunk& k = ch[ci];
-            if (gqa) {
-                QkvRopeArgs qa{(bf16*)c->q + (size_t)k.m0 * da, (bf16*)c->k + (size_t)k.m0 * dkv, (bf16*)c->vt, c->cos_tab, c->sin_tab, L, Lpad, da, Hl};
-                qa.chunked = nch > 1; qa.row0 = k.m0;
-                qa.n_kv_heads = Hkv; qa.bias = (const bf16*)l.bqkv;
-                if (gemm_bf16(EPI_QKVGQA, xn + (size_t)k.m0 * d, d, (const bf16*)l.wqkv, d, k.Mc, da + 2 * dkv, d, nullptr, 0, nullptr, 0, &qa, k.s))
-                    return -1;
-                continue;
-            }
-            QkvRopeArgs qa{(bf16*)c->q + (size_t)k.m0 * da, (bf16*)c->k + (size_t)k.m0 * da, (bf16*)c->vt, c->cos_tab, c->sin_tab, L, Lpad, da, Hl};
+            QkvRopeArgs qa{(bf16*)c->q + (size_t)k.m0 * da, (bf16*)c->k + (size_t)k.m0 * dkv, (bf16*)c->vt, c->cos_tab, c->sin_tab, L, Lpad, da, Hl};
             qa.chunked = nch > 1; qa.row0 = k.m0;
-            if (gemm_bf16(EPI_QKVROPE, xn + (size_t)k.m0 * d, d, (const bf16*)l.wqkv, d, k.Mc, 3 * da, d, nullptr, 0, nullptr, 0, &qa, k.s)) return -1;
+            if (gqa) { qa.n_kv_heads = Hkv; qa.bias = (const bf16*)l.bqkv; }
+            const int epi = gqa ? EPI_QKVGQA : EPI_QKVROPE;
+            if (f8 ? gemm_fp8(epi, xq_chunk[ci][c->rank], d, xs_chunk[ci][c->rank], l8->wqkv, d, l8->sqkv, k.Mc, da + 2 * dkv, d, nullptr, 0,
+                              nullptr, 0, &qa, k.s)
+                   : gemm_bf16(epi, xn + (size_t)k.m0 * d, d, (const bf16*)l.wqkv, d, k.Mc, da + 2 * dkv, d, nullptr, 0, nullptr, 0, &qa, k.s))
+                return -1;
         }
         // attention mixes all rows: both chunks' q / k / v^T must be complete, and it must be complete before either chain goes on
         if (join()) return -1;
@@ -483,11 +543,25 @@ MMDP_API int mmdp_tp_forward(const mmdp_tp_ctx* c, const int64_t* ids, int B, in
             const Chunk& k = ch[ci];
             const bf16* att = (const bf16*)c->att + (size_t)k.m0 * da;
             bf16* h = (bf16*)c->h + (size_t)k.m0 * ffl;
-            if (gemm_bf16(EPI_F32, att, da, (const bf16*)l.wo, da, k.Mc, d, da, nullptr, d, nullptr, 0, nullptr, k.s, &k.sc[0])) return -1;
-            if (reduce(ci, 0, l.ff_norm, e1)) return -1;
-            if (gemm_bf16(EPI_SWIGLU, xn + (size_t)k.m0 * d, d, (const bf16*)l.w13, d, k.Mc, 2 * ffl, d, h, ffl, nullptr, 0, nullptr, k.s)) return -1;
-            if (gemm_bf16(EPI_F32, h, ffl, (const bf16*)l.w2, ffl, k.Mc, d, ffl, nullptr, d, nullptr, 0, nullptr, k.s, &k.sc[1])) return -1;
-            if (reduce(ci, 1, li + 1 < c->n_layers ? c->layers[li + 1].attn_norm : c->ln_f, e2)) return -1;
+            const bool last = li + 1 == c->n_layers;
+            if (f8) {
+                uint8_t* q8;
+                float* s8;
+                if (quant_local(ci, att, da, &q8, &s8)) return -1;
+                if (gemm_fp8(EPI_F32, q8, da, s8, l8->wo, da, l8->so, k.Mc, d, da, nullptr, d, nullptr, 0, nullptr, k.s, &k.sc[0])) return -1;
+                if (reduce(ci, 0, l.ff_norm, e1, true)) return -1;
+                if (gemm_fp8(EPI_SWIGLU, xq_chunk[ci][c->rank], d, xs_chunk[ci][c->rank], l8->w13, d, l8->s13, k.Mc, 2 * ffl, d, h, ffl, nullptr,
+                             0, nullptr, k.s))
+                    return -1;
+                if (quant_local(ci, h, ffl, &q8, &s8)) return -1;
+                if (gemm_fp8(EPI_F32, q8, ffl, s8, l8->w2, ffl, l8->s2, k.Mc, d, ffl, nullptr, d, nullptr, 0, nullptr, k.s, &k.sc[1])) return -1;
+            } else {
+                if (gemm_bf16(EPI_F32, att, da, (const bf16*)l.wo, da, k.Mc, d, da, nullptr, d, nullptr, 0, nullptr, k.s, &k.sc[0])) return -1;
+                if (reduce(ci, 0, l.ff_norm, e1, false)) return -1;
+                if (gemm_bf16(EPI_SWIGLU, xn + (size_t)k.m0 * d, d, (const bf16*)l.w13, d, k.Mc, 2 * ffl, d, h, ffl, nullptr, 0, nullptr, k.s)) return -1;
+                if (gemm_bf16(EPI_F32, h, ffl, (const bf16*)l.w2, ffl, k.Mc, d, ffl, nullptr, d, nullptr, 0, nullptr, k.s, &k.sc[1])) return -1;
+            }
+            if (reduce(ci, 1, last ? c->ln_f : c->layers[li + 1].attn_norm, e2, f8 && !last)) return -1;
         }
     }
     if (join()) return -1;

@@ -11,6 +11,8 @@
 // fresh fragment that is then promoted into the fp32 master accumulator with the activation scale (the fp8 wgmma
 // accumulator keeps fewer bits than fp32; the promotion bounds that error to one k-block). Two 64-register fragments per
 // thread are why the tile is 128 wide. No split-K tail and no CTA-pair variant: every tile runs its whole K loop.
+// EPI_F32 (tensor-parallel partial sums of the row-parallel linears) stores the scaled fp32 accumulators, or pushes each row to
+// the rank that owns it (GemmScatter; gemm_epilogue_tile decides the owner per row, so a 128-row tile may span two owners).
 #include "gemm_epilogue.cuh"
 
 namespace mmdp {
@@ -19,13 +21,7 @@ namespace mmdp {
 // quantiser: one warp per (row, group) with lane l holding elements 4l + 128t of the group; for the activation groups
 // (G = 128) one half-warp per group with 16-byte loads, so that twice the bytes per thread are in flight
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float absmax4(uint2 v, float m) {
-    return fmaxf(fmaxf(m, fmaxf(fabsf(bf16_lo(v.x)), fabsf(bf16_hi(v.x)))), fmaxf(fabsf(bf16_lo(v.y)), fabsf(bf16_hi(v.y))));
-}
-__device__ __forceinline__ uint32_t quant4(uint2 v, float s) {
-    return pack_e4m3x4(__fdiv_rn(bf16_lo(v.x), s), __fdiv_rn(bf16_hi(v.x), s), __fdiv_rn(bf16_lo(v.y), s), __fdiv_rn(bf16_hi(v.y), s));
-}
-
+// (absmax4 / quant4: ptx.cuh)
 __global__ void __launch_bounds__(256) quantize_fp8_kernel(const __nv_bfloat16* __restrict__ x, int ldx, int rows, int K, int G,
                                                            uint8_t* __restrict__ q, int ldq, float* __restrict__ scales) {
     const int ng = K / G;
@@ -202,6 +198,9 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             }
             gemm_epilogue_tile<EPI, BN>(p, acc, m_blk, n_blk, rit0, c0);
         }
+        if constexpr (EPI == EPI_F32) {
+            if (p.scat_R > 0) __threadfence_system();  // the pushed rows are visible to their owners before this grid completes
+        }
     }
 }
 
@@ -221,7 +220,11 @@ static int launch_gemm_fp8(const CUtensorMap& tmA, const CUtensorMap& tmB, const
 }
 
 int gemm_fp8(int epi, const uint8_t* A, int lda, const float* sa, const uint8_t* W, int ldw, const float* sw, int M, int N,
-             int K, __nv_bfloat16* C, int ldc, const __nv_bfloat16* resid, int ldr, const QkvRopeArgs* qa, cudaStream_t stream) {
+             int K, __nv_bfloat16* C, int ldc, const __nv_bfloat16* resid, int ldr, const QkvRopeArgs* qa, cudaStream_t stream,
+             const GemmScatter* scat) {
+    if (scat && epi != EPI_F32) return set_error("gemm_fp8: the scatter epilogue belongs to EPI_F32");
+    if (scat && (scat->rows_per_rank <= 0 || scat->slot < 0 || scat->slot > 7 || (M + scat->rows_per_rank - 1) / scat->rows_per_rank > 8))
+        return set_error("gemm_fp8: bad scatter layout");
     if (M <= 0 || N <= 0 || K <= 0) return set_error("gemm_fp8: empty problem");
     if (!A || !W || !sa || !sw) return set_error("gemm_fp8: null operand or scale pointer");
     if (K % kF8BK) return set_error("gemm_fp8: K must be a multiple of 128 (the activation scale group)");
@@ -233,6 +236,9 @@ int gemm_fp8(int epi, const uint8_t* A, int lda, const float* sa, const uint8_t*
             break;
         case EPI_RESID:
             if (!C || !resid || (ldc % 8) || (ldr % 8) || (N % 8)) return set_error("gemm_fp8: bad residual epilogue args");
+            break;
+        case EPI_F32:
+            if ((!C && !scat) || (ldc % 4) || (N % 4)) return set_error("gemm_fp8: fp32 output needs ldc/N multiples of 4");
             break;
         case EPI_SWIGLU:
             if (!C || (ldc % 8) || (N % kF8BN)) return set_error("gemm_fp8: swiglu needs N %% 128 == 0 (gate/up interleaved in 64-row blocks)");
@@ -262,6 +268,10 @@ int gemm_fp8(int epi, const uint8_t* A, int lda, const float* sa, const uint8_t*
         p.pos_map = qa->pos_map; p.Tq = qa->Tq; p.row0 = qa->row0; p.seg_pos = qa->seg_pos;
         p.n_kv_heads = qa->n_kv_heads; p.bias = qa->bias;
     }
+    if (scat) {
+        for (int r = 0; r < 8; ++r) p.scat_dst[r] = scat->dst[r];
+        p.scat_R = scat->rows_per_rank; p.scat_slot = scat->slot;
+    }
     const Fp8Scales sc{sa, sw};
     const int tiles = ((M + kF8BM - 1) / kF8BM) * ((N + kF8BN - 1) / kF8BN);
     const int grid = tiles < num_sms() ? tiles : num_sms();
@@ -271,6 +281,7 @@ int gemm_fp8(int epi, const uint8_t* A, int lda, const float* sa, const uint8_t*
     switch (epi) {
         case EPI_PLAIN: return launch_gemm_fp8<EPI_PLAIN>(tmA, tmB, p, sc, grid, stream);
         case EPI_RESID: return launch_gemm_fp8<EPI_RESID>(tmA, tmB, p, sc, grid, stream);
+        case EPI_F32: return launch_gemm_fp8<EPI_F32>(tmA, tmB, p, sc, grid, stream);
         case EPI_SWIGLU: return launch_gemm_fp8<EPI_SWIGLU>(tmA, tmB, p, sc, grid, stream);
         case EPI_QKVROPE_PACKED: return launch_gemm_fp8<EPI_QKVROPE_PACKED>(tmA, tmB, p, sc, grid, stream);
         case EPI_QKVGQA: return launch_gemm_fp8<EPI_QKVGQA>(tmA, tmB, p, sc, grid, stream);

@@ -153,11 +153,13 @@ int gemm_group_m(int M);
 
 // FP8 (e4m3) path (fp8.cu). quantize_fp8: x bf16 [rows, K] (row stride ldx) -> q e4m3 [rows, K] (row stride ldq) and fp32
 // scales [K / group][rows]; group divides K and is a multiple of 128. gemm_fp8: A e4m3 [M, K] with scales sa [K/128][M],
-// W e4m3 [N, K] with row scales sw [N]; epilogues PLAIN, RESID, SWIGLU (W13 interleaved in 64-row blocks), QKVROPE.
+// W e4m3 [N, K] with row scales sw [N]; epilogues PLAIN, RESID, SWIGLU (W13 interleaved in 64-row blocks), QKVROPE / QKVGQA,
+// and F32 (fp32 C, or with `scat` each row pushed to the rank that owns it, as gemm_bf16's scatter).
 int quantize_fp8(const __nv_bfloat16* x, int ldx, int rows, int K, int group, uint8_t* q, int ldq, float* scales,
                  cudaStream_t stream);
 int gemm_fp8(int epi, const uint8_t* A, int lda, const float* sa, const uint8_t* W, int ldw, const float* sw, int M, int N,
-             int K, __nv_bfloat16* C, int ldc, const __nv_bfloat16* resid, int ldr, const QkvRopeArgs* qa, cudaStream_t stream);
+             int K, __nv_bfloat16* C, int ldc, const __nv_bfloat16* resid, int ldr, const QkvRopeArgs* qa, cudaStream_t stream,
+             const GemmScatter* scat = nullptr);
 
 int gemm_pair_mode();
 void set_gemm_pair_mode(int on);
@@ -207,5 +209,10 @@ int lfq_decode(const int64_t* ids, float* zq, int B, int N, int bits, cudaStream
 int tp_reduce_norm(const float* recv_local, int rows_per_rank, int n_src, uint16_t* const* xn, uint32_t* const* flags, int n_ranks,
                    int my_rank, uint16_t* x_shard, const uint16_t* w, int row0, int nrows, int d, float eps, uint32_t epoch,
                    unsigned int* done_counter, cudaStream_t stream);
+// FP8 form: the normalised rows go to every rank as e4m3 bytes xq[r] [rows, d] plus 1 x 128 group scales xs[r] [d / 128][ld_s],
+// bitwise what quantize_fp8(group 128) makes of the bf16 rows tp_reduce_norm would store
+int tp_reduce_norm_fp8(const float* recv_local, int rows_per_rank, int n_src, uint8_t* const* xq, float* const* xs, int ld_s,
+                       uint32_t* const* flags, int n_ranks, int my_rank, uint16_t* x_shard, const uint16_t* w, int row0, int nrows,
+                       int d, float eps, uint32_t epoch, unsigned int* done_counter, cudaStream_t stream);
 
 }  // namespace mmdp

@@ -268,4 +268,13 @@ __device__ __forceinline__ uint32_t pack_e4m3x4(float a0, float a1, float a2, fl
     return (uint32_t)lo | ((uint32_t)hi << 16);
 }
 
+// the e4m3 quantiser's two steps on four bf16 values packed in a uint2 (the activation / weight quantiser of fp8.cu and the
+// fused FP8 broadcast of tp_collective.cu): running amax of |x|, and e4m3(x / s) with IEEE division
+__device__ __forceinline__ float absmax4(uint2 v, float m) {
+    return fmaxf(fmaxf(m, fmaxf(fabsf(bf16_lo(v.x)), fabsf(bf16_hi(v.x)))), fmaxf(fabsf(bf16_lo(v.y)), fabsf(bf16_hi(v.y))));
+}
+__device__ __forceinline__ uint32_t quant4(uint2 v, float s) {
+    return pack_e4m3x4(__fdiv_rn(bf16_lo(v.x), s), __fdiv_rn(bf16_hi(v.x), s), __fdiv_rn(bf16_lo(v.y), s), __fdiv_rn(bf16_hi(v.y), s));
+}
+
 }  // namespace mmdp

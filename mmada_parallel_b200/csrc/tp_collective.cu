@@ -18,6 +18,12 @@
 // phase 1 of all ranks in tp_wait_kernel. Flags carry a monotonically increasing epoch, so they never need resetting.
 // Buffer reuse is safe with TWO partial buffers used alternately (a rank can only overwrite a partial buffer two
 // collectives later, after it has itself passed the next phase-0 barrier, which every peer joins only after its reads).
+//
+// FP8 form (tp_reduce_norm_fp8, the tensor-parallel forward with e4m3 block linears): the normalised bf16 row is not stored
+// but quantised on the spot, exactly as quantize_fp8 (fp8.cu, group 128) would quantise it - a 128-column group is the 16
+// consecutive threads of a half-warp, amax by half-warp shuffles, s = amax / 448 (1 for an all-zero group), q = e4m3(x / s) -
+// and the e4m3 bytes plus the group scales go to every rank: d + d/32 bytes per row instead of 2d, and no rank has to
+// quantise the replicated activations itself before its next column-parallel GEMM.
 #include "mmdp_internal.h"
 #include "ptx.cuh"
 
@@ -69,8 +75,16 @@ __device__ __forceinline__ void tp_wait_flags(const uint32_t* flags_local, int p
     __syncthreads();
 }
 
-template <int NV>  // d <= 2048 * NV columns (d % 8 == 0): every thread owns up to NV groups of 8 consecutive columns
-__global__ void __launch_bounds__(kTpThreads) tp_reduce_norm_kernel(TpReduceArgs a) {
+// destination of the FP8 form: every rank's e4m3 activation buffer and its scales (peer-mapped)
+struct TpFp8Out {
+    uint8_t* q[kTpMaxRanks];  // [rows, d] e4m3
+    float* s[kTpMaxRanks];    // [d / 128][ld_s] fp32, row index contiguous (the layout of quantize_fp8)
+    int ld_s;
+};
+
+// d <= 2048 * NV columns (d % 8 == 0; d % 128 == 0 for F8): every thread owns up to NV groups of 8 consecutive columns
+template <int NV, bool F8>
+__device__ __forceinline__ void tp_reduce_norm_body(const TpReduceArgs& a, const TpFp8Out& f) {
     const int tid = threadIdx.x;
     // the phase-0 rendezvous (every rank's partial sums are complete) has been passed by tp_rendezvous_kernel, the previous
     // launch in this stream: this grid never spins
@@ -145,10 +159,28 @@ __global__ void __launch_bounds__(kTpThreads) tp_reduce_norm_kernel(TpReduceArgs
             const float n1 = bf16_round(__fmul_rn(xv[t][2 * j + 1], rstd));
             o[j] = pack_bf16x2(__fmul_rn(bf16_lo(ww[j]), n0), __fmul_rn(bf16_hi(ww[j]), n1));
         }
-        const uint4 ov = make_uint4(o[0], o[1], o[2], o[3]);
+        if constexpr (F8) {
+            // quantize_fp8_g128_kernel's arithmetic on the bf16 row: half-warp h of the warp holds one 128-column group
+            const uint2 v0 = make_uint2(o[0], o[1]), v1 = make_uint2(o[2], o[3]);
+            float amax = absmax4(v1, absmax4(v0, 0.f));
+            const unsigned half_mask = 0xffffu << (tid & 16);
 #pragma unroll
-        for (int r = 0; r < kTpMaxRanks; ++r)
-            if (r < a.n_ranks) *reinterpret_cast<uint4*>(a.xn[r] + grow + c) = ov;  // the all-gather: P2P stores
+            for (int sh = 8; sh > 0; sh >>= 1) amax = fmaxf(amax, __shfl_xor_sync(half_mask, amax, sh));
+            const float sc = amax > 0.f ? __fdiv_rn(amax, 448.0f) : 1.0f;
+            const uint2 qv = make_uint2(quant4(v0, sc), quant4(v1, sc));
+            const size_t si = (size_t)(c >> 7) * f.ld_s + a.row0 + lrow;
+#pragma unroll
+            for (int r = 0; r < kTpMaxRanks; ++r)
+                if (r < a.n_ranks) {  // the all-gather of the e4m3 row and its scales: P2P stores
+                    *reinterpret_cast<uint2*>(f.q[r] + grow + c) = qv;
+                    if ((tid & 15) == 0) f.s[r][si] = sc;
+                }
+        } else {
+            const uint4 ov = make_uint4(o[0], o[1], o[2], o[3]);
+#pragma unroll
+            for (int r = 0; r < kTpMaxRanks; ++r)
+                if (r < a.n_ranks) *reinterpret_cast<uint4*>(a.xn[r] + grow + c) = ov;  // the all-gather: P2P stores
+        }
     }
     // phase 1: when the LAST CTA of this rank has stored its rows, tell every rank that this rank's rows have landed
     __threadfence_system();
@@ -161,6 +193,16 @@ __global__ void __launch_bounds__(kTpThreads) tp_reduce_norm_kernel(TpReduceArgs
     }
     __syncthreads();
     if (s_last && tid < a.n_ranks) st_release_sys(a.flags[tid] + 1 * kTpMaxRanks + a.my_rank, a.epoch);
+}
+
+template <int NV>
+__global__ void __launch_bounds__(kTpThreads) tp_reduce_norm_kernel(TpReduceArgs a) {
+    tp_reduce_norm_body<NV, false>(a, TpFp8Out{});
+}
+
+template <int NV>
+__global__ void __launch_bounds__(kTpThreads) tp_reduce_norm_fp8_kernel(TpReduceArgs a, TpFp8Out f) {
+    tp_reduce_norm_body<NV, true>(a, f);
 }
 
 // Phase 0 of a collective, ONE small CTA: tell every rank that this rank has reached the collective - its partial sums are
@@ -185,9 +227,10 @@ __global__ void tp_wait_kernel(const uint32_t* flags_local, int phase, int n_ran
     pdl_launch_dependents();  // after the wait, see tp_rendezvous_kernel
 }
 
-int tp_reduce_norm(const float* recv_local, int rows_per_rank, int n_src, uint16_t* const* xn, uint32_t* const* flags, int n_ranks,
-                   int my_rank, uint16_t* x_shard, const uint16_t* w, int row0, int nrows, int d, float eps, uint32_t epoch,
-                   unsigned int* done_counter, cudaStream_t stream) {
+// f8 == nullptr: the bf16 form (xn); otherwise the FP8 form into f8's buffers (xn unused)
+static int tp_reduce_launch(const float* recv_local, int rows_per_rank, int n_src, uint16_t* const* xn, const TpFp8Out* f8,
+                            uint32_t* const* flags, int n_ranks, int my_rank, uint16_t* x_shard, const uint16_t* w, int row0, int nrows,
+                            int d, float eps, uint32_t epoch, unsigned int* done_counter, cudaStream_t stream) {
     if (n_ranks < 1 || n_ranks > kTpMaxRanks || my_rank < 0 || my_rank >= n_ranks) return set_error("tp_reduce_norm: bad rank layout");
     if (n_src != 0 && n_src != n_ranks) return set_error("tp_reduce_norm: n_src must be 0 (no partial sums) or n_ranks");
     if (n_src && (!recv_local || nrows > rows_per_rank)) return set_error("tp_reduce_norm: receive buffer / rows_per_rank mismatch");
@@ -196,7 +239,7 @@ int tp_reduce_norm(const float* recv_local, int rows_per_rank, int n_src, uint16
     TpReduceArgs a{};
     for (int r = 0; r < n_ranks; ++r) {
         a.part[r] = n_src ? recv_local + (size_t)r * rows_per_rank * d : nullptr;
-        a.xn[r] = reinterpret_cast<__nv_bfloat16*>(xn[r]);
+        a.xn[r] = f8 ? nullptr : reinterpret_cast<__nv_bfloat16*>(xn[r]);
         a.flags[r] = flags[r];
     }
     a.n_ranks = n_ranks; a.n_src = n_src; a.my_rank = my_rank;
@@ -212,13 +255,25 @@ int tp_reduce_norm(const float* recv_local, int rows_per_rank, int n_src, uint16
         MMDP_CUDA(launch_ex(tp_rendezvous_kernel, dim3(1), dim3(32), 0, stream, pdl, false, fp, my_rank, n_ranks, epoch));
     }
     {
-    // bytes this rank moves: reads n_src fp32 rows + x, writes x + n_ranks bf16 rows
-    LaunchScope ls(LK_ROW, (double)nrows * d * (4.0 * n_src + 4.0 + 2.0 * n_ranks), stream);
-    switch ((d + 2047) / 2048) {
-        case 1: e = launch_ex(tp_reduce_norm_kernel<1>, dim3(nrows), dim3(kTpThreads), 0, stream, pdl, false, a); break;
-        case 2: e = launch_ex(tp_reduce_norm_kernel<2>, dim3(nrows), dim3(kTpThreads), 0, stream, pdl, false, a); break;
-        case 3: e = launch_ex(tp_reduce_norm_kernel<3>, dim3(nrows), dim3(kTpThreads), 0, stream, pdl, false, a); break;
-        default: e = launch_ex(tp_reduce_norm_kernel<4>, dim3(nrows), dim3(kTpThreads), 0, stream, pdl, false, a); break;
+    // bytes this rank moves: reads n_src fp32 rows + x, writes x + n_ranks bf16 rows (FP8: n_ranks e4m3 rows + their scales)
+    const double out_row = f8 ? d + d / 32.0 : 2.0 * d;
+    LaunchScope ls(LK_ROW, (double)nrows * (d * (4.0 * n_src + 4.0) + out_row * n_ranks), stream);
+    const int nv = (d + 2047) / 2048;
+    if (f8) {
+        const TpFp8Out& f = *f8;
+        switch (nv) {
+            case 1: e = launch_ex(tp_reduce_norm_fp8_kernel<1>, dim3(nrows), dim3(kTpThreads), 0, stream, pdl, false, a, f); break;
+            case 2: e = launch_ex(tp_reduce_norm_fp8_kernel<2>, dim3(nrows), dim3(kTpThreads), 0, stream, pdl, false, a, f); break;
+            case 3: e = launch_ex(tp_reduce_norm_fp8_kernel<3>, dim3(nrows), dim3(kTpThreads), 0, stream, pdl, false, a, f); break;
+            default: e = launch_ex(tp_reduce_norm_fp8_kernel<4>, dim3(nrows), dim3(kTpThreads), 0, stream, pdl, false, a, f); break;
+        }
+    } else {
+        switch (nv) {
+            case 1: e = launch_ex(tp_reduce_norm_kernel<1>, dim3(nrows), dim3(kTpThreads), 0, stream, pdl, false, a); break;
+            case 2: e = launch_ex(tp_reduce_norm_kernel<2>, dim3(nrows), dim3(kTpThreads), 0, stream, pdl, false, a); break;
+            case 3: e = launch_ex(tp_reduce_norm_kernel<3>, dim3(nrows), dim3(kTpThreads), 0, stream, pdl, false, a); break;
+            default: e = launch_ex(tp_reduce_norm_kernel<4>, dim3(nrows), dim3(kTpThreads), 0, stream, pdl, false, a); break;
+        }
     }
     }
     MMDP_CUDA(e);
@@ -226,6 +281,31 @@ int tp_reduce_norm(const float* recv_local, int rows_per_rank, int n_src, uint16
     LaunchScope ls2(LK_ROW, 0.0, stream);
     MMDP_CUDA(launch_ex(tp_wait_kernel, dim3(1), dim3(32), 0, stream, pdl, false, (const uint32_t*)flags[my_rank], 1, n_ranks, epoch));
     return 0;
+}
+
+int tp_reduce_norm(const float* recv_local, int rows_per_rank, int n_src, uint16_t* const* xn, uint32_t* const* flags, int n_ranks,
+                   int my_rank, uint16_t* x_shard, const uint16_t* w, int row0, int nrows, int d, float eps, uint32_t epoch,
+                   unsigned int* done_counter, cudaStream_t stream) {
+    return tp_reduce_launch(recv_local, rows_per_rank, n_src, xn, nullptr, flags, n_ranks, my_rank, x_shard, w, row0, nrows, d, eps,
+                            epoch, done_counter, stream);
+}
+
+int tp_reduce_norm_fp8(const float* recv_local, int rows_per_rank, int n_src, uint8_t* const* xq, float* const* xs, int ld_s,
+                       uint32_t* const* flags, int n_ranks, int my_rank, uint16_t* x_shard, const uint16_t* w, int row0, int nrows,
+                       int d, float eps, uint32_t epoch, unsigned int* done_counter, cudaStream_t stream) {
+    if (!xq || !xs) return set_error("tp_reduce_norm_fp8: null buffer array");
+    if (d % 128) return set_error("tp_reduce_norm_fp8: d must be a multiple of 128 (the activation scale group)");
+    if (ld_s < row0 + nrows) return set_error("tp_reduce_norm_fp8: the scale stride %d is below the rows %d", ld_s, row0 + nrows);
+    if (n_ranks < 1 || n_ranks > kTpMaxRanks) return set_error("tp_reduce_norm: bad rank layout");
+    TpFp8Out f{};
+    for (int r = 0; r < n_ranks; ++r) {
+        if (!xq[r] || !xs[r]) return set_error("tp_reduce_norm_fp8: null buffer of rank %d", r);
+        f.q[r] = xq[r];
+        f.s[r] = xs[r];
+    }
+    f.ld_s = ld_s;
+    return tp_reduce_launch(recv_local, rows_per_rank, n_src, nullptr, &f, flags, n_ranks, my_rank, x_shard, w, row0, nrows, d, eps,
+                            epoch, done_counter, stream);
 }
 
 }  // namespace mmdp

@@ -15,6 +15,12 @@ GPUs of one node. The reference has no tensor parallelism (SURVEY.md 2c); this f
   * every rank gathers the logits slices it needs (NCCL all_gather, once per forward) and runs the SAME sampling kernels on
     the same noise (identical generator seeds), so the id sequence stays in sync without broadcasts.
 
+`precision="fp8"` runs the four block linears in e4m3 as the single-GPU FP8 context does (DESIGN §3 "FP8 under tensor
+parallel"): every weight is quantised whole (one scale per row over the full K) and then sliced (shard_state_dict_fp8), the
+reduce before a column-parallel linear broadcasts e4m3 rows and their 1 x 128 group scales (`mmdp_tp_reduce_norm_fp8`), att and
+h are quantised locally before the row-parallel FP8 GEMMs that push fp32 partial rows (`mmdp_gemm_fp8_f32_scatter`), and ln_f
+after the last layer stays bf16 for the LM head.
+
 `collective="nccl"` keeps round 1's formulation (fp32 `dist.all_reduce` + `mmdp_resid_add_f32` + `mmdp_rmsnorm` between the
 kernels) as the measured baseline of the peer-memory path (bench.py --tp --tp-collective nccl).
 Buffers shared between the ranks are plain cudaMalloc allocations exported with CUDA IPC (`mmdp_ipc_export/import`); the
@@ -89,6 +95,46 @@ def shard_state_dict(sd: Dict[str, torch.Tensor], n_layers: int, n_heads: int, r
     return out
 
 
+def _interleave64(gate: torch.Tensor, up: torch.Tensor) -> torch.Tensor:
+    """Rows (or row scales) of the FP8 W13: 64-row blocks of gate and up alternating (the FP8 GEMM's tile is 128 wide)."""
+    nb = gate.shape[0] // 64
+    return torch.stack([gate.reshape(nb, 64, *gate.shape[1:]), up.reshape(nb, 64, *up.shape[1:])], dim=1).reshape(2 * nb * 64, *gate.shape[1:])
+
+
+def shard_state_dict_fp8(sd: Dict[str, torch.Tensor], n_layers: int, n_heads: int, rank: int, tp: int, quantize, *,
+                         n_kv_heads: Optional[int] = None) -> Dict[str, torch.Tensor]:
+    """Rank `rank`'s FP8 shard of the four block linears of every layer. `quantize(w)` maps a full bf16 weight [N, K] to its
+    e4m3 bytes (uint8 [N, K]) and row scales (fp32 [N]) with one scale per row over the full K (mmdp_quantize_fp8 with group =
+    K, or oracle.fp8's restatement); every weight is quantised WHOLE and then sliced, so that each byte and scale a rank holds is
+    bitwise a slice of the single-GPU FP8 context's weights:
+      * column-parallel (q/k/v_proj as shard_state_dict's rows, ff_proj / up_proj): the rank's rows and their row scales; W13
+        interleaves 64-row blocks of gate and up inside the shard (the FP8 GEMM's 128-wide SwiGLU tile);
+      * row-parallel (attn_out, ff_out): the rank's K-columns of the bytes and the FULL row scales [d].
+    Keys `blocks.i.` + wqkv8 / sqkv, wo8 / so, w13_8 / s13, w2_8 / s2."""
+    g = lambda n: sd["model.transformer." + n] if ("model.transformer." + n) in sd else sd[n]
+    da = (n_heads // tp) * 128
+    kv0, n_kv_local = kv_shard(n_heads, n_kv_heads or n_heads, rank, tp)
+    sl, kv = slice(rank * da, (rank + 1) * da), slice(kv0 * 128, (kv0 + n_kv_local) * 128)
+    out = {}
+    for i in range(n_layers):
+        p = f"blocks.{i}."
+        (qq, sq), (qk, sk), (qv, sv) = (quantize(g(p + n + ".weight")) for n in ("q_proj", "k_proj", "v_proj"))
+        out[p + "wqkv8"] = torch.cat([qq[sl], qk[kv], qv[kv]]).contiguous()
+        out[p + "sqkv"] = torch.cat([sq[sl], sk[kv], sv[kv]]).contiguous()
+        qo, so = quantize(g(p + "attn_out.weight"))
+        out[p + "wo8"], out[p + "so"] = qo[:, sl].contiguous(), so.contiguous()
+        (q1, s1), (q3, s3) = quantize(g(p + "ff_proj.weight")), quantize(g(p + "up_proj.weight"))
+        ff = q1.shape[0]
+        if (ff // tp) % 128:
+            raise ValueError("mlp_hidden / tp must be a multiple of 128 (SwiGLU tile interleave)")
+        fs = slice(rank * (ff // tp), (rank + 1) * (ff // tp))
+        out[p + "w13_8"] = _interleave64(q1[fs], q3[fs]).contiguous()
+        out[p + "s13"] = _interleave64(s1[fs], s3[fs]).contiguous()
+        q2, s2 = quantize(g(p + "ff_out.weight"))
+        out[p + "w2_8"], out[p + "s2"] = q2[:, fs].contiguous(), s2.contiguous()
+    return out
+
+
 def rows_per_rank(M: int, tp: int) -> int:
     return (M + tp - 1) // tp
 
@@ -159,7 +205,10 @@ class TensorParallelLLaDA:
 
     def __init__(self, config, state_dict: Dict[str, torch.Tensor], tp_rank: int, tp_size: int, group=None,
                  max_seq_len: Optional[int] = None, max_batch: int = 1, device: str = "cuda:0", text_vocab_size: int = 126356,
-                 codebook_size: int = 8192, collective: str = "p2p", chunks: Optional[int] = None):
+                 codebook_size: int = 8192, collective: str = "p2p", chunks: Optional[int] = None, precision: str = "bf16"):
+        if precision not in ("bf16", "fp8"):
+            raise ValueError(f"precision must be 'bf16' or 'fp8' (e4m3 block linears), not {precision!r}")
+        self.precision = precision
         if not torch.cuda.is_available():
             raise _lib.MmdpError("mmada_parallel_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         if collective not in ("p2p", "nccl"):
@@ -198,7 +247,13 @@ class TensorParallelLLaDA:
         self.max_batch = max_batch
         sh = shard_state_dict(state_dict, self.n_layers, self.n_heads, tp_rank, tp_size, text_vocab_size, codebook_size,
                               n_kv_heads=self.n_kv_heads, qkv_bias=self.qkv_bias)
+        fp8 = precision == "fp8"
+        if fp8:  # the bf16 linears are not kept: their FP8 shards replace them
+            sh = {k: v for k, v in sh.items() if k.split(".")[-1] not in ("wqkv", "wo", "w13", "w2")}
         self.w = {k: v.detach().to(device=self.device, dtype=torch.bfloat16).contiguous() for k, v in sh.items()}
+        if fp8:
+            self.w.update(shard_state_dict_fp8(state_dict, self.n_layers, self.n_heads, tp_rank, tp_size, self._quantize_rows,
+                                               n_kv_heads=self.n_kv_heads))
         cos, sin = rope_tables(128, float(g("rope_theta", 10000.0)), self.max_seq_len)
         self.cos, self.sin = cos.to(self.device), sin.to(self.device)
         M, d, bf = self.max_batch * self.max_seq_len, self.d_model, dict(dtype=torch.bfloat16, device=self.device)
@@ -207,6 +262,11 @@ class TensorParallelLLaDA:
         self.k = torch.empty((M, self.kv_local * 128), **bf)
         self.att = torch.empty((M, self.d_attn), **bf)
         self.h = torch.empty((M, self.ff_local), **bf)
+        if fp8:
+            # the e4m3 copy of the input of a linear quantised on this rank (att, h; the NCCL path also xn) and its scales
+            ka = max(self.d_model, self.d_attn, self.ff_local)
+            self.a8 = torch.empty(M * ka, dtype=torch.uint8, device=self.device)
+            self.a8s = torch.empty(M * ka // 128, dtype=torch.float32, device=self.device)
         self.vt = None
         self._vt_key = None
         if self.collective == "p2p":
@@ -225,6 +285,12 @@ class TensorParallelLLaDA:
                 self._chunk_state.append(st)
             self._xn = _SharedBuffer(M * d * 2, tp_rank, tp_size, group)
             self.xn = torch.as_tensor(_DeviceArray(self._xn.own, M * d, "<u2"), device=self.device).view(torch.bfloat16).view(M, d)
+            self._xq = None
+            if fp8:
+                # the e4m3 activation buffer every reduce but the last broadcasts into: [M, d] bytes, then M * d / 128 scales
+                self._xq = _SharedBuffer(M * d + M * (d // 128) * 4, tp_rank, tp_size, group)
+                self._xq_arr = (C.c_void_p * tp_size)(*self._xq.ptrs)
+                self._xs_arr = (C.c_void_p * tp_size)(*[q + M * d for q in self._xq.ptrs])
             self.x = self._chunk_state[0]["x"]
             self._epoch = 0
             torch.cuda.synchronize()
@@ -235,7 +301,7 @@ class TensorParallelLLaDA:
             self.part = torch.empty((M, d), dtype=torch.float32, device=self.device)
 
     def __del__(self):
-        shared = [getattr(self, "_xn", None)]
+        shared = [getattr(self, "_xn", None), getattr(self, "_xq", None)]
         for st in getattr(self, "_chunk_state", []):
             shared += st["recv"] + [st["flags"]]
         for b in shared:
@@ -247,6 +313,16 @@ class TensorParallelLLaDA:
 
     def eval(self):
         return self
+
+    def _quantize_rows(self, w: torch.Tensor):
+        """One full weight [N, K] -> (e4m3 bytes uint8 [N, K], row scales fp32 [N]) on this rank's device: mmdp_quantize_fp8 with
+        one group per row, the quantisation of the single-GPU FP8 context's mmdp_model_set_weight."""
+        q, s = _lib.quantize_fp8(w.detach().to(device=self.device, dtype=torch.bfloat16).contiguous(), group=w.shape[1])
+        return q.view(torch.uint8), s[0]
+
+    def _quantize_input(self, a: torch.Tensor, M: int, K: int, s):
+        """The bf16 input [M, K] of an FP8 linear -> e4m3 bytes and 1 x 128 group scales in a8 / a8s."""
+        check(lib.mmdp_quantize_fp8(ptr(a), K, M, K, 128, ptr(self.a8), K, ptr(self.a8s), s))
 
     def _allreduce(self, t: torch.Tensor):
         if self.tp > 1:
@@ -269,6 +345,8 @@ class TensorParallelLLaDA:
         d, s, w = self.d_model, stream_ptr(), self.w
         scale = 1.0 / math.sqrt(128.0)
         x, xn = self.x, self.xn
+        if self.precision == "fp8":
+            return self._layers_nccl_fp8(B, L, M, Lpad)
         for i in range(self.n_layers):
             p = f"blocks.{i}."
             check(lib.mmdp_rmsnorm(ptr(x), d, None, ptr(w[p + "attn_norm"]), ptr(xn), d, M, d, self.rms_eps, s))
@@ -293,6 +371,35 @@ class TensorParallelLLaDA:
             self._allreduce(self.part[:M])
             check(lib.mmdp_resid_add_f32(ptr(x), d, ptr(self.part), d, M, d, s))
 
+    def _layers_nccl_fp8(self, B: int, L: int, M: int, Lpad: int):
+        """_layers_nccl with the four linears in FP8: each bf16 input is quantised (1 x 128 groups) right before its GEMM."""
+        d, s, w, da, ffl = self.d_model, stream_ptr(), self.w, self.d_attn, self.ff_local
+        scale = 1.0 / math.sqrt(128.0)
+        x, xn, a8, a8s = self.x, self.xn, ptr(self.a8), ptr(self.a8s)
+        for i in range(self.n_layers):
+            p = f"blocks.{i}."
+            check(lib.mmdp_rmsnorm(ptr(x), d, None, ptr(w[p + "attn_norm"]), ptr(xn), d, M, d, self.rms_eps, s))
+            self._quantize_input(xn, M, d, s)
+            check(lib.mmdp_qkv_rope_tp_fp8(a8, d, a8s, ptr(w[p + "wqkv8"]), ptr(w[p + "sqkv"]), ptr(w.get(p + "bqkv")), M, d, self.h_local,
+                                           self.kv_local, L, Lpad, ptr(self.cos), ptr(self.sin), ptr(self.q), ptr(self.k), ptr(self.vt), s))
+            if self.gqa:
+                check(lib.mmdp_attention_gqa(ptr(self.q), ptr(self.k), ptr(self.vt), ptr(self.att), B, None, self.h_local, self.kv_local,
+                                             L, Lpad, scale, s))
+            else:
+                check(lib.mmdp_attention(ptr(self.q), ptr(self.k), ptr(self.vt), ptr(self.att), B, self.h_local, L, Lpad, scale, s))
+            self._quantize_input(self.att, M, da, s)
+            check(lib.mmdp_gemm_fp8_f32(a8, da, a8s, ptr(w[p + "wo8"]), da, ptr(w[p + "so"]), M, d, da, ptr(self.part), d, s))
+            self._allreduce(self.part[:M])
+            check(lib.mmdp_resid_add_f32(ptr(x), d, ptr(self.part), d, M, d, s))
+            check(lib.mmdp_rmsnorm(ptr(x), d, None, ptr(w[p + "ff_norm"]), ptr(xn), d, M, d, self.rms_eps, s))
+            self._quantize_input(xn, M, d, s)
+            check(lib.mmdp_gemm_fp8(EPI_SWIGLU, a8, d, a8s, ptr(w[p + "w13_8"]), d, ptr(w[p + "s13"]), M, 2 * ffl, d, ptr(self.h), ffl,
+                                    None, 0, s))
+            self._quantize_input(self.h, M, ffl, s)
+            check(lib.mmdp_gemm_fp8_f32(a8, ffl, a8s, ptr(w[p + "w2_8"]), ffl, ptr(w[p + "s2"]), M, d, ffl, ptr(self.part), d, s))
+            self._allreduce(self.part[:M])
+            check(lib.mmdp_resid_add_f32(ptr(x), d, ptr(self.part), d, M, d, s))
+
     def _native_ctx(self, B: int, L: int):
         """The C-side description of this rank (mmdp_tp_ctx): built once per (B, L) - the V^T buffer depends on it."""
         key = (B, L)
@@ -300,11 +407,17 @@ class TensorParallelLLaDA:
             return self._ctx
         w = self.w
         layers = (_lib.TpLayer * self.n_layers)()
+        fp8 = self.precision == "fp8"
+        layers8 = (_lib.TpLayerFp8 * self.n_layers)() if fp8 else None
         for i in range(self.n_layers):
             p = f"blocks.{i}."
-            for name, t in (("wqkv", w[p + "wqkv"]), ("wo", w[p + "wo"]), ("w13", w[p + "w13"]), ("w2", w[p + "w2"]),
-                            ("attn_norm", w[p + "attn_norm"]), ("ff_norm", w[p + "ff_norm"])):
-                setattr(layers[i], name, t.data_ptr())
+            names = ("attn_norm", "ff_norm") if fp8 else ("wqkv", "wo", "w13", "w2", "attn_norm", "ff_norm")
+            for name in names:
+                setattr(layers[i], name, w[p + name].data_ptr())
+            if fp8:
+                for name, key in (("wqkv", "wqkv8"), ("wo", "wo8"), ("w13", "w13_8"), ("w2", "w2_8"), ("sqkv", "sqkv"), ("so", "so"),
+                                  ("s13", "s13"), ("s2", "s2")):
+                    setattr(layers8[i], name, w[p + key].data_ptr())
             if self.qkv_bias:
                 layers[i].bqkv = w[p + "bqkv"].data_ptr()
         c = _lib.TpCtx()
@@ -316,6 +429,12 @@ class TensorParallelLLaDA:
         c.cos_tab, c.sin_tab = self.cos.data_ptr(), self.sin.data_ptr()
         c.q, c.k, c.att, c.h, c.vt = self.q.data_ptr(), self.k.data_ptr(), self.att.data_ptr(), self.h.data_ptr(), self.vt.data_ptr()
         c.xn = C.cast(self._xn.array, C.POINTER(C.c_void_p))
+        if fp8:
+            c.precision = _lib.PRECISION_FP8
+            c.layers_fp8 = layers8
+            c.xq = C.cast(self._xq_arr, C.POINTER(C.c_void_p))
+            c.xq_scales = C.cast(self._xs_arr, C.POINTER(C.c_void_p))
+            c.a8, c.a8_scales = self.a8.data_ptr(), self.a8s.data_ptr()
         split = chunk_split(B * L) if self.chunks == 2 else [B * L]
         c.n_chunks = len(split)
         c.chunk_rows0 = split[0]
@@ -326,7 +445,7 @@ class TensorParallelLLaDA:
             c.chunk[ci].recv[1] = C.cast(st["recv"][1].array, C.POINTER(C.c_void_p))
             c.chunk[ci].flags = C.cast(st["flags"].array, C.POINTER(C.c_void_p))
             c.chunk[ci].done_counter = st["done"].data_ptr()
-        self._ctx, self._ctx_layers, self._ctx_key = c, layers, key   # (keep the layer array alive)
+        self._ctx, self._ctx_layers, self._ctx_key = c, (layers, layers8), key   # (keep the layer arrays alive)
         return c
 
     def _final_norm(self, ids: torch.Tensor) -> torch.Tensor:
