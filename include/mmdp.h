@@ -170,10 +170,23 @@ typedef struct mmdp_tp_ctx {
                                                     [m0, m0 + Mc)) at offset m0 * d / 128, laid out [d / 128][Mc] */
     uint8_t* a8;                                 /* FP8: local e4m3 copy of att / h, M * max(d_attn, ff_local) bytes */
     float* a8_scales;                            /* FP8: its scales, M * max(d_attn, ff_local) / 128 fp32 */
+    /* Packed forwards (mmdp_tp_forward_packed): the device row map, int2 [max_rows] ((sequence, position) of every packed row),
+     * and the capacities the segment table is checked against: max_rows = the rows every work buffer above holds, rope_len = the
+     * positions of cos_tab / sin_tab. A zero-initialised field leaves mmdp_tp_forward unchanged and refuses packed forwards. */
+    struct { void* seg_pos; int32_t max_rows; int32_t rope_len; } packed;
 } mmdp_tp_ctx;
 /* epoch0: the last epoch used so far; the call uses epoch0 + 1 ... epoch0 + 2 * n_layers + 1 on every chunk's flags (returned
  * through *epoch_out). With two chunks the call uses an internal second stream, forked from and joined back into `stream`. */
 MMDP_API int mmdp_tp_forward(const mmdp_tp_ctx* c, const int64_t* ids, int B, int L, uint32_t epoch0, uint32_t* epoch_out, void* stream);
+/* mmdp_tp_forward over a PACKED variable-length batch: n_seg (1..64) sequences of seg_len[i] (host int32, 1..packed.rope_len) rows
+ * laid end to end in M = sum seg_len <= packed.max_rows rows of ids. Each sequence is computed as if it were alone: attention stays
+ * inside it and its positions restart at 0 (the contract of mmdp_model_forward_packed). Row ownership, the scatter GEMMs, the
+ * reduces, the epochs and the row chunks are those of mmdp_tp_forward over the M packed rows; a chunk boundary may fall inside a
+ * sequence (chunk_rows0 in (0, M)). vt is [n_seg, n_kv_heads_local, 128, Lpad], Lpad = max seg_len rounded up to 8, and the columns
+ * [seg_len[i], Lpad) of block i must be finite zeros. Bad sizes, and a chunk that leaves a rank without rows, return an error before
+ * anything is launched. On return every rank's xn holds ln_f(x) of the M packed rows. */
+MMDP_API int mmdp_tp_forward_packed(const mmdp_tp_ctx* c, const int64_t* ids, int n_seg, const int32_t* seg_len, uint32_t epoch0,
+                                    uint32_t* epoch_out, void* stream);
 
 /* ---- epilogues of mmdp_gemm_bf16 ----------------------------------------------------------------------------- */
 #define MMDP_EPI_PLAIN 0   /* C = bf16(A W^T)                                 nn.Linear, modeling_llada.py:1402      */
@@ -240,6 +253,18 @@ MMDP_API int mmdp_qkv_rope_tp_gqa(const uint16_t* A, int lda, const uint16_t* Wq
 MMDP_API int mmdp_qkv_rope_tp_fp8(const uint8_t* A, int lda, const float* sa, const uint8_t* Wqkv, const float* sw, const uint16_t* bias,
                                   int M, int d_model, int n_heads_local, int n_kv_heads_local, int L, int Lpad, const float* cos_tab,
                                   const float* sin_tab, uint16_t* q, uint16_t* k, uint16_t* vt, void* stream);
+
+/* Packed form of the shard's projection (mmdp_qkv_rope_tp / _gqa / _fp8 over a packed variable-length batch): n_seg (1..64)
+ * sequences of seg_len[i] (host int32) rows end to end, M = sum seg_len rows of A; positions restart at 0 in every sequence.
+ * precision MMDP_PRECISION_BF16: A bf16 [M, d_model] (row stride lda), Wqkv bf16, sa / sw NULL; MMDP_PRECISION_FP8: A e4m3 with
+ * scales sa [d_model / 128][M], Wqkv e4m3 with row scales sw, as mmdp_qkv_rope_tp_fp8. A multi-head shard without a bias runs the
+ * multi-head epilogue, any other the grouped-query one. q [M, 128 n_heads_local], k [M, 128 n_kv_heads_local] (RoPE applied);
+ * vt [n_seg, n_kv_heads_local, 128, Lpad] with Lpad >= every seg_len, Lpad % 8 == 0 (pad columns untouched). row_map: caller-given
+ * device workspace of M int2, filled by the call. Attention on the result: mmdp_attention_gqa(..., n_seg, seg_len, ...). */
+MMDP_API int mmdp_qkv_rope_tp_packed(int precision, const void* A, int lda, const float* sa, const void* Wqkv, const float* sw,
+                                     const uint16_t* bias, int d_model, int n_heads_local, int n_kv_heads_local, int n_seg,
+                                     const int32_t* seg_len, int Lpad, const float* cos_tab, const float* sin_tab, uint16_t* q,
+                                     uint16_t* k, uint16_t* vt, void* row_map, void* stream);
 
 /* x = bf16(bf16(partial) + x): residual add of an fp32 partial-sum buffer that was all-reduced across tensor-parallel ranks
  * (keeps the reference's rounding points: nn.Linear output -> bf16, then the residual add -> bf16). */

@@ -63,6 +63,11 @@ class TpChunk(C.Structure):
     _fields_ = [("x_shard", C.c_void_p), ("recv", C.POINTER(C.c_void_p) * 2), ("flags", C.POINTER(C.c_void_p)), ("done_counter", C.c_void_p)]
 
 
+class TpPacked(C.Structure):
+    """mmdp_tp_ctx.packed: the device row map int2 [max_rows] of packed forwards and the capacities it is checked against."""
+    _fields_ = [("seg_pos", C.c_void_p), ("max_rows", C.c_int32), ("rope_len", C.c_int32)]
+
+
 class TpCtx(C.Structure):
     _fields_ = [("d_model", C.c_int32), ("n_heads_local", C.c_int32), ("ff_local", C.c_int32), ("n_layers", C.c_int32),
                 ("n_ranks", C.c_int32), ("rank", C.c_int32), ("rms_eps", C.c_float), ("layers", C.POINTER(TpLayer)),
@@ -70,7 +75,8 @@ class TpCtx(C.Structure):
                 ("q", C.c_void_p), ("k", C.c_void_p), ("att", C.c_void_p), ("h", C.c_void_p), ("vt", C.c_void_p),
                 ("xn", C.POINTER(C.c_void_p)), ("n_chunks", C.c_int32), ("chunk_rows0", C.c_int32), ("chunk", TpChunk * 2),
                 ("n_kv_heads_local", C.c_int32), ("precision", C.c_int32), ("layers_fp8", C.POINTER(TpLayerFp8)),
-                ("xq", C.POINTER(C.c_void_p)), ("xq_scales", C.POINTER(C.c_void_p)), ("a8", C.c_void_p), ("a8_scales", C.c_void_p)]
+                ("xq", C.POINTER(C.c_void_p)), ("xq_scales", C.POINTER(C.c_void_p)), ("a8", C.c_void_p), ("a8_scales", C.c_void_p),
+                ("packed", TpPacked)]
 
 
 class ModelConfig(C.Structure):
@@ -103,6 +109,7 @@ SIGNATURES = {
     "mmdp_ipc_import": (_i, [_vp, C.POINTER(_vp)]),
     "mmdp_ipc_close": (_i, [_vp]),
     "mmdp_tp_forward": (_i, [C.POINTER(TpCtx), _vp, _i, _i, C.c_uint32, C.POINTER(C.c_uint32), _vp]),
+    "mmdp_tp_forward_packed": (_i, [C.POINTER(TpCtx), _vp, _i, _vp, C.c_uint32, C.POINTER(C.c_uint32), _vp]),
     "mmdp_gemm_f32_scatter": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),
     "mmdp_tp_reduce_norm": (_i, [_vp, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _i, _f, C.c_uint32, _vp, _vp]),
     "mmdp_gemm_fp8_f32": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _i, _i, _vp, _i, _vp]),
@@ -116,6 +123,7 @@ SIGNATURES = {
     "mmdp_qkv_rope_gqa": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mmdp_qkv_rope_tp_gqa": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mmdp_qkv_rope_tp_fp8": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "mmdp_qkv_rope_tp_packed": (_i, [_i, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mmdp_resid_add_f32": (_i, [_vp, _i, _vp, _i, _i, _i, _vp]),
     "mmdp_attention": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp]),
     "mmdp_attention_packed": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _f, _vp]),

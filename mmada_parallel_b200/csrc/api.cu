@@ -42,6 +42,20 @@ int packed_row_map(const SegTable& segs, int2* seg_pos, cudaStream_t stream) {
     return 0;
 }
 
+// sequence table of a packed call: n_seg in [1, kMaxSegs], every length in [1, max_len]; returns the longest length, or -1
+static int seg_table(const char* who, int n_seg, const int32_t* seg_len, int max_len, SegTable* segs) {
+    if (!seg_len || n_seg <= 0 || n_seg > kMaxSegs) return set_error("%s: %d sequences (1 to %d)", who, n_seg, kMaxSegs);
+    segs->n = n_seg;
+    segs->start[0] = 0;
+    int Lmax = 0;
+    for (int i = 0; i < n_seg; ++i) {
+        if (seg_len[i] <= 0 || seg_len[i] > max_len) return set_error("%s: sequence %d has length %d (1 to %d)", who, i, seg_len[i], max_len);
+        segs->start[i + 1] = segs->start[i] + seg_len[i];
+        Lmax = seg_len[i] > Lmax ? seg_len[i] : Lmax;
+    }
+    return Lmax;
+}
+
 // Last-block row windows of a packed forward: sequence s (packed rows [start[s], start[s + 1])) keeps its positions [lo[s], hi[s]),
 // stored as compact rows [out0[s], out0[s + 1]), the windows of all sequences end to end.
 struct WinTable {
@@ -239,6 +253,37 @@ MMDP_API int mmdp_qkv_rope_tp_fp8(const uint8_t* A, int lda, const float* sa, co
                     &qa, (cudaStream_t)stream);
 }
 
+MMDP_API int mmdp_qkv_rope_tp_packed(int precision, const void* A, int lda, const float* sa, const void* Wqkv, const float* sw,
+                                     const uint16_t* bias, int d_model, int n_heads_local, int n_kv_heads_local, int n_seg,
+                                     const int32_t* seg_len, int Lpad, const float* cos_tab, const float* sin_tab, uint16_t* q,
+                                     uint16_t* k, uint16_t* vt, void* row_map, void* stream) {
+    if (!A || !Wqkv || !row_map) return set_error("mmdp_qkv_rope_tp_packed: null argument");
+    if (precision != MMDP_PRECISION_BF16 && precision != MMDP_PRECISION_FP8)
+        return set_error("mmdp_qkv_rope_tp_packed: unknown precision %d", precision);
+    if (precision == MMDP_PRECISION_FP8 && (!sa || !sw)) return set_error("mmdp_qkv_rope_tp_packed: FP8 needs the scales sa and sw");
+    SegTable segs{};
+    const int Lmax = seg_table("mmdp_qkv_rope_tp_packed", n_seg, seg_len, Lpad, &segs);
+    if (Lmax < 0) return -1;
+    if (Lpad % 8) return set_error("mmdp_qkv_rope_tp_packed: Lpad=%d must be a multiple of 8", Lpad);
+    if (n_heads_local <= 0 || n_kv_heads_local <= 0 || n_heads_local % n_kv_heads_local || d_model <= 0)
+        return set_error("mmdp_qkv_rope_tp_packed: n_kv_heads_local=%d must divide n_heads_local=%d", n_kv_heads_local, n_heads_local);
+    const int M = segs.start[n_seg], da = n_heads_local * 128;
+    QkvRopeArgs qa{(bf16*)q, (bf16*)k, (bf16*)vt, cos_tab, sin_tab, Lmax, Lpad, da, n_heads_local};
+    qa.seg_pos = (const int2*)row_map;
+    int epi = EPI_QKVROPE_PACKED, N = 3 * da;
+    if (n_kv_heads_local != n_heads_local || bias) {
+        epi = EPI_QKVGQA_PACKED;
+        N = da + 2 * 128 * n_kv_heads_local;
+        qa.n_kv_heads = n_kv_heads_local;
+        qa.bias = (const bf16*)bias;
+    }
+    if (packed_row_map(segs, (int2*)row_map, (cudaStream_t)stream)) return -1;
+    if (precision == MMDP_PRECISION_FP8)
+        return gemm_fp8(epi, (const uint8_t*)A, lda, sa, (const uint8_t*)Wqkv, d_model, sw, M, N, d_model, nullptr, 0, nullptr, 0, &qa,
+                        (cudaStream_t)stream);
+    return gemm_bf16(epi, (const bf16*)A, lda, (const bf16*)Wqkv, d_model, M, N, d_model, nullptr, 0, nullptr, 0, &qa, (cudaStream_t)stream);
+}
+
 MMDP_API int mmdp_resid_add_f32(uint16_t* x, int ldx, const float* partial, int ldp, int M, int d, void* stream) {
     return resid_add_f32((bf16*)x, ldx, partial, ldp, M, d, (cudaStream_t)stream);
 }
@@ -428,15 +473,19 @@ static int tp_side(TpSide** out) {
     return 0;
 }
 
-MMDP_API int mmdp_tp_forward(const mmdp_tp_ctx* c, const int64_t* ids, int B, int L, uint32_t epoch0, uint32_t* epoch_out, void* stream) {
-    if (!c || !ids || !epoch_out) return set_error("mmdp_tp_forward: null argument");
+// The tensor-parallel body of mmdp_tp_forward (segs == nullptr: B sequences of L rows) and mmdp_tp_forward_packed (segs: the
+// packed batch, whose sizes the caller has checked; L = the longest sequence). Only the QKV epilogue, the attention launch and the
+// V^T layout see the sequences; everything else works on the M rows.
+static int tp_forward(const mmdp_tp_ctx* c, const int64_t* ids, const SegTable* segs, int B, int L, uint32_t epoch0, uint32_t* epoch_out,
+                      void* stream) {
     cudaStream_t s0 = (cudaStream_t)stream;
     const int d = c->d_model, Hl = c->n_heads_local, da = Hl * 128, ffl = c->ff_local, tp = c->n_ranks;
     // kv heads of this rank's shard: 0 = Hl (the multi-head shard)
     const int Hkv = c->n_kv_heads_local ? c->n_kv_heads_local : Hl, dkv = Hkv * 128;
     if (Hkv <= 0 || Hkv > Hl || Hl % Hkv)
         return set_error("mmdp_tp_forward: n_kv_heads_local=%d must divide n_heads_local=%d", c->n_kv_heads_local, Hl);
-    const int M = B * L, Lpad = ((L + 7) / 8) * 8;
+    const int M = segs ? segs->start[segs->n] : B * L, Lpad = ((L + 7) / 8) * 8;
+    const int2* seg_pos = segs ? (const int2*)c->packed.seg_pos : nullptr;
     const int nch = c->n_chunks == 2 ? 2 : 1;
     if (c->precision != MMDP_PRECISION_BF16 && c->precision != MMDP_PRECISION_FP8)
         return set_error("mmdp_tp_forward: unknown precision %d", c->precision);
@@ -460,6 +509,9 @@ MMDP_API int mmdp_tp_forward(const mmdp_tp_ctx* c, const int64_t* ids, int B, in
         k.nrows = k.Mc - k.row0 < k.R ? k.Mc - k.row0 : k.R;
         if (k.nrows < 1 || k.Mc - (tp - 1) * k.R < 1)
             return set_error("mmdp_tp_forward: %d rows cannot be split over %d ranks with at least one row each", k.Mc, tp);
+    }
+    for (int ci = 0; ci < nch; ++ci) {  // the chunks' shared buffers are read only once every chunk's split is checked
+        Chunk& k = ch[ci];
         k.s = ci == 0 ? s0 : side->s1;
         for (int b = 0; b < 2; ++b) {
             k.sc[b] = GemmScatter{};
@@ -511,6 +563,7 @@ MMDP_API int mmdp_tp_forward(const mmdp_tp_ctx* c, const int64_t* ids, int B, in
         return 0;
     };
     const bf16* xn = (const bf16*)c->xn[c->rank];
+    if (segs && packed_row_map(*segs, (int2*)c->packed.seg_pos, s0)) return -1;
     if (fork()) return -1;
     ++epoch;
     for (int ci = 0; ci < nch; ++ci) {
@@ -526,9 +579,11 @@ MMDP_API int mmdp_tp_forward(const mmdp_tp_ctx* c, const int64_t* ids, int B, in
         for (int ci = 0; ci < nch; ++ci) {
             const Chunk& k = ch[ci];
             QkvRopeArgs qa{(bf16*)c->q + (size_t)k.m0 * da, (bf16*)c->k + (size_t)k.m0 * dkv, (bf16*)c->vt, c->cos_tab, c->sin_tab, L, Lpad, da, Hl};
-            qa.chunked = nch > 1; qa.row0 = k.m0;
+            // packed: chunk ci's GEMM row r is packed row m0 + r, so it reads the row map from m0 as q / k start at m0
+            if (segs) qa.seg_pos = seg_pos + k.m0;
+            else { qa.chunked = nch > 1; qa.row0 = k.m0; }
             if (gqa) { qa.n_kv_heads = Hkv; qa.bias = (const bf16*)l.bqkv; }
-            const int epi = gqa ? EPI_QKVGQA : EPI_QKVROPE;
+            const int epi = segs ? (gqa ? EPI_QKVGQA_PACKED : EPI_QKVROPE_PACKED) : (gqa ? EPI_QKVGQA : EPI_QKVROPE);
             if (f8 ? gemm_fp8(epi, xq_chunk[ci][c->rank], d, xs_chunk[ci][c->rank], l8->wqkv, d, l8->sqkv, k.Mc, da + 2 * dkv, d, nullptr, 0,
                               nullptr, 0, &qa, k.s)
                    : gemm_bf16(epi, xn + (size_t)k.m0 * d, d, (const bf16*)l.wqkv, d, k.Mc, da + 2 * dkv, d, nullptr, 0, nullptr, 0, &qa, k.s))
@@ -536,7 +591,9 @@ MMDP_API int mmdp_tp_forward(const mmdp_tp_ctx* c, const int64_t* ids, int B, in
         }
         // attention mixes all rows: both chunks' q / k / v^T must be complete, and it must be complete before either chain goes on
         if (join()) return -1;
-        if (attention_fwd((const bf16*)c->q, (const bf16*)c->k, (const bf16*)c->vt, (bf16*)c->att, B, Hl, L, Lpad, scale, s0, 0, Hkv)) return -1;
+        if (segs ? attention_packed_fwd((const bf16*)c->q, (const bf16*)c->k, (const bf16*)c->vt, (bf16*)c->att, *segs, Hl, Lpad, scale, s0, Hkv)
+                 : attention_fwd((const bf16*)c->q, (const bf16*)c->k, (const bf16*)c->vt, (bf16*)c->att, B, Hl, L, Lpad, scale, s0, 0, Hkv))
+            return -1;
         if (fork()) return -1;
         const uint32_t e1 = ++epoch, e2 = ++epoch;
         for (int ci = 0; ci < nch; ++ci) {
@@ -567,6 +624,24 @@ MMDP_API int mmdp_tp_forward(const mmdp_tp_ctx* c, const int64_t* ids, int B, in
     if (join()) return -1;
     *epoch_out = epoch;
     return 0;
+}
+
+MMDP_API int mmdp_tp_forward(const mmdp_tp_ctx* c, const int64_t* ids, int B, int L, uint32_t epoch0, uint32_t* epoch_out, void* stream) {
+    if (!c || !ids || !epoch_out) return set_error("mmdp_tp_forward: null argument");
+    return tp_forward(c, ids, nullptr, B, L, epoch0, epoch_out, stream);
+}
+
+MMDP_API int mmdp_tp_forward_packed(const mmdp_tp_ctx* c, const int64_t* ids, int n_seg, const int32_t* seg_len, uint32_t epoch0,
+                                    uint32_t* epoch_out, void* stream) {
+    if (!c || !ids || !epoch_out) return set_error("mmdp_tp_forward_packed: null argument");
+    if (!c->packed.seg_pos || c->packed.max_rows <= 0 || c->packed.rope_len <= 0)
+        return set_error("mmdp_tp_forward_packed: the context has no packed row map (packed.seg_pos, max_rows, rope_len)");
+    SegTable segs{};
+    const int Lmax = seg_table("mmdp_tp_forward_packed", n_seg, seg_len, c->packed.rope_len, &segs);
+    if (Lmax < 0) return -1;
+    if (segs.start[n_seg] > c->packed.max_rows)
+        return set_error("mmdp_tp_forward_packed: %d packed rows exceed the workspace of %d", segs.start[n_seg], c->packed.max_rows);
+    return tp_forward(c, ids, &segs, n_seg, Lmax, epoch0, epoch_out, stream);
 }
 
 MMDP_API void mmdp_prof_enable(int on) { prof_enable(on); }

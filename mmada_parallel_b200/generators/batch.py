@@ -12,7 +12,9 @@ computed as if it were alone. A global step advances every unfinished request by
   3. one packed forward over the unconditional sequences of the requests in an image step (one or two per request, each of
      its request's length), after their text steps like in the reference;
   4. each request's image step (`image_sample`).
-Requests with fewer steps drop out. A set of more than `max_batch` sequences runs as several packed forwards.
+Requests with fewer steps drop out. A set of more than `max_batch` sequences runs as several packed forwards. The
+tensor-parallel model (tensor_parallel.TensorParallelLLaDA) serves batches too: every rank calls generate_ti2ti_batch with the
+same requests and generator seeds, as it calls generate_ti2ti.
 The sampling stays per request: each draws from its own generator in the order generate_ti2ti does, so the draws of one
 request do not depend on its neighbours. Still-masked image tokens are drawn from the global CPU RNG after the loop, in request
 order, like sequential calls would.
@@ -66,9 +68,11 @@ def _bind(model, requests) -> List[dict]:
         a = dict(a.arguments)
         check_request(model, a["input_ids"], a["remasking"])
         args.append(a)
-    if not hasattr(model, "forward_rows_packed"):
-        raise TypeError("generate_ti2ti_batch needs a model with packed forwards (mmada_parallel_b200.model."
-                        "LLaDAForMultiModalGeneration); the tensor-parallel model serves one request at a time")
+    # a model with packed forwards exposes its capacity; an object without it (e.g. never constructed) is not a usable model
+    if not hasattr(model, "forward_rows_packed") or not all(hasattr(model, k) for k in ("max_batch", "max_seq_len")):
+        raise TypeError("generate_ti2ti_batch needs a constructed model with packed forwards and their capacity (max_batch, "
+                        "max_seq_len): mmada_parallel_b200.model.LLaDAForMultiModalGeneration or "
+                        "mmada_parallel_b200.tensor_parallel.TensorParallelLLaDA")
     seen = set()
     for i, a in enumerate(args):
         g = a["generator"]
@@ -166,7 +170,8 @@ def generate_ti2ti_batch(model, requests: Sequence[dict]) -> list:
             image_sample(states[i], g, noise[i], a["text_steps"], a["temperature"], a["cfg_scale"], a["cfg_img"],
                          a["noise_schedule"], a["text_vocab_size"], a["codebook_size"], a["_trace"])
     finals = [st.ids[0].cpu() for st in states]
-    model.raise_device_errors()
+    if hasattr(model, "raise_device_errors"):  # the tensor-parallel model has no device error flags (as in generate_ti2ti)
+        model.raise_device_errors()
     results = []
     for st, a, final in zip(states, args, finals):
         image_tokens, text, _ = extract_results(st, final, a["tokenizer"], a["text_vocab_size"], a["codebook_size"])

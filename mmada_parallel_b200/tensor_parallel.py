@@ -21,6 +21,13 @@ reduce before a column-parallel linear broadcasts e4m3 rows and their 1 x 128 gr
 h are quantised locally before the row-parallel FP8 GEMMs that push fp32 partial rows (`mmdp_gemm_fp8_f32_scatter`), and ln_f
 after the last layer stays bf16 for the LM head.
 
+Packed batches (`forward_rows_packed`, the call `generators.batch.generate_ti2ti_batch` makes) lay several sequences end to end
+in one forward, each computed as if it were alone, exactly as the single-GPU model's packed forward does (DESIGN §3 "Packed
+batches under tensor parallel"): only the QKV epilogue, the attention launch and the V^T layout see the sequences; row ownership,
+the scatter GEMMs, the reduces and the row chunks work on the packed rows. `max_batch = N` sizes every per-rank work buffer for N
+full-length sequences: q, k, att, h, xn (and in FP8 the e4m3 copy xq and a8) and the receive buffers (2 per chunk, fp32 rows of
+this rank's share) all grow linearly with N.
+
 `collective="nccl"` keeps round 1's formulation (fp32 `dist.all_reduce` + `mmdp_resid_add_f32` + `mmdp_rmsnorm` between the
 kernels) as the measured baseline of the peer-memory path (bench.py --tp --tp-collective nccl).
 Buffers shared between the ranks are plain cudaMalloc allocations exported with CUDA IPC (`mmdp_ipc_export/import`); the
@@ -269,36 +276,50 @@ class TensorParallelLLaDA:
             self.a8s = torch.empty(M * ka // 128, dtype=torch.float32, device=self.device)
         self.vt = None
         self._vt_key = None
+        # packed forwards: the device row map of the packed rows, and their own V^T buffer [max_batch][kv_local][128][Lpad] (allocated
+        # on the first packed forward) with the pad-rule bookkeeping of csrc/api.cu's vt_prepare: _pvt_Lpad = the column stride it was
+        # last zeroed for, _pvt_len[s] = the columns of block s written since then
+        self._row_map = torch.empty((M, 2), dtype=torch.int32, device=self.device)
+        self._pvt = None
+        self._pvt_Lpad, self._pvt_len = 0, [0] * self.max_batch
         if self.collective == "p2p":
-            if M < tp_size:
-                raise ValueError("the workspace must hold at least one row per rank")
-            # per row chunk (see chunk_split): receive buffers [tp][R][d] fp32 (slot r <- rank r's partial rows for the rows this
-            # rank owns), used alternately; flags; this rank's rows of the residual stream. Chunk 0 is sized for the whole
-            # workspace (a short sequence runs as one chunk), chunk 1 for half of it.
-            self._chunk_state = []
-            for ci in range(self._alloc_chunks):
-                rows = M if ci == 0 else (M + 1) // 2          # chunk 1 never holds more than half of the rows (chunk_split)
-                R = rows_per_rank(rows, tp_size)
-                st = {"recv": [_SharedBuffer(tp_size * R * d * 4, tp_rank, tp_size, group) for _ in range(2)],
-                      "flags": _SharedBuffer(2 * 8 * 4, tp_rank, tp_size, group),
-                      "x": torch.empty((R, d), **bf), "done": torch.zeros(1, dtype=torch.int32, device=self.device)}
-                self._chunk_state.append(st)
-            self._xn = _SharedBuffer(M * d * 2, tp_rank, tp_size, group)
-            self.xn = torch.as_tensor(_DeviceArray(self._xn.own, M * d, "<u2"), device=self.device).view(torch.bfloat16).view(M, d)
-            self._xq = None
-            if fp8:
-                # the e4m3 activation buffer every reduce but the last broadcasts into: [M, d] bytes, then M * d / 128 scales
-                self._xq = _SharedBuffer(M * d + M * (d // 128) * 4, tp_rank, tp_size, group)
-                self._xq_arr = (C.c_void_p * tp_size)(*self._xq.ptrs)
-                self._xs_arr = (C.c_void_p * tp_size)(*[q + M * d for q in self._xq.ptrs])
-            self.x = self._chunk_state[0]["x"]
-            self._epoch = 0
-            torch.cuda.synchronize()
-            dist.barrier(group=group)  # every rank has mapped every buffer before the first peer access
+            self._init_peer_buffers(group)
         else:
             self.x = torch.empty((M, d), **bf)
             self.xn = torch.empty((M, d), **bf)
             self.part = torch.empty((M, d), dtype=torch.float32, device=self.device)
+
+    def _init_peer_buffers(self, group) -> None:
+        """The peer-memory state of the "p2p" collective (csrc/tp_collective.cu): receive buffers, flags and the shared activation
+        buffers of every row chunk, exported to and imported from the other ranks of `group`. Every rank calls it together."""
+        M, d, tp_size, tp_rank = self.Mmax, self.d_model, self.tp, self.rank
+        fp8 = self.precision == "fp8"
+        bf = dict(dtype=torch.bfloat16, device=self.device)
+        if M < tp_size:
+            raise ValueError("the workspace must hold at least one row per rank")
+        # per row chunk (see chunk_split): receive buffers [tp][R][d] fp32 (slot r <- rank r's partial rows for the rows this
+        # rank owns), used alternately; flags; this rank's rows of the residual stream. Chunk 0 is sized for the whole
+        # workspace (a short sequence runs as one chunk), chunk 1 for half of it.
+        self._chunk_state = []
+        for ci in range(self._alloc_chunks):
+            rows = M if ci == 0 else (M + 1) // 2          # chunk 1 never holds more than half of the rows (chunk_split)
+            R = rows_per_rank(rows, tp_size)
+            st = {"recv": [_SharedBuffer(tp_size * R * d * 4, tp_rank, tp_size, group) for _ in range(2)],
+                  "flags": _SharedBuffer(2 * 8 * 4, tp_rank, tp_size, group),
+                  "x": torch.empty((R, d), **bf), "done": torch.zeros(1, dtype=torch.int32, device=self.device)}
+            self._chunk_state.append(st)
+        self._xn = _SharedBuffer(M * d * 2, tp_rank, tp_size, group)
+        self.xn = torch.as_tensor(_DeviceArray(self._xn.own, M * d, "<u2"), device=self.device).view(torch.bfloat16).view(M, d)
+        self._xq = None
+        if fp8:
+            # the e4m3 activation buffer every reduce but the last broadcasts into: [M, d] bytes, then M * d / 128 scales
+            self._xq = _SharedBuffer(M * d + M * (d // 128) * 4, tp_rank, tp_size, group)
+            self._xq_arr = (C.c_void_p * tp_size)(*self._xq.ptrs)
+            self._xs_arr = (C.c_void_p * tp_size)(*[q + M * d for q in self._xq.ptrs])
+        self.x = self._chunk_state[0]["x"]
+        self._epoch = 0
+        torch.cuda.synchronize()
+        dist.barrier(group=group)  # every rank has mapped every buffer before the first peer access
 
     def __del__(self):
         shared = [getattr(self, "_xn", None), getattr(self, "_xq", None)]
@@ -339,18 +360,35 @@ class TensorParallelLLaDA:
         out.view(n, self.tp, c).copy_(buf.permute(1, 0, 2))
 
     # ------------------------------------------------------------------------------------------------------------------
-    def _layers_nccl(self, B: int, L: int, M: int, Lpad: int):
+    def _packed_qkv_attention(self, p: str, packed, Lpad: int, a8=None, a8s=None):
+        """QKV + RoPE and attention of layer prefix `p` over the packed batch packed = (n_seg, host int32 lengths) on the NCCL path:
+        mmdp_qkv_rope_tp_packed on xn (bf16) or on its e4m3 copy a8 / a8s (FP8), then the packed attention."""
+        d, s, w = self.d_model, stream_ptr(), self.w
+        n, lens = packed
+        if a8 is None:
+            prec, a, sa, wq, sw = _lib.PRECISION_BF16, ptr(self.xn), None, ptr(w[p + "wqkv"]), None
+        else:
+            prec, a, sa, wq, sw = _lib.PRECISION_FP8, a8, a8s, ptr(w[p + "wqkv8"]), ptr(w[p + "sqkv"])
+        check(lib.mmdp_qkv_rope_tp_packed(prec, a, d, sa, wq, sw, ptr(w.get(p + "bqkv")), d, self.h_local, self.kv_local, n, lens, Lpad,
+                                          ptr(self.cos), ptr(self.sin), ptr(self.q), ptr(self.k), ptr(self._pvt), ptr(self._row_map), s))
+        check(lib.mmdp_attention_gqa(ptr(self.q), ptr(self.k), ptr(self._pvt), ptr(self.att), n, lens, self.h_local, self.kv_local, 0,
+                                     Lpad, 1.0 / math.sqrt(128.0), s))
+
+    def _layers_nccl(self, B: int, L: int, M: int, Lpad: int, packed=None):
         """Round 1's formulation, kept as the measured baseline (`collective="nccl"`): fp32 partial sums stored locally,
-        `dist.all_reduce` between the kernels, then the residual add and the RMSNorm as separate launches."""
+        `dist.all_reduce` between the kernels, then the residual add and the RMSNorm as separate launches. packed: (n_seg, host
+        int32 lengths) of a packed batch of M rows (B, L unused), or None."""
         d, s, w = self.d_model, stream_ptr(), self.w
         scale = 1.0 / math.sqrt(128.0)
         x, xn = self.x, self.xn
         if self.precision == "fp8":
-            return self._layers_nccl_fp8(B, L, M, Lpad)
+            return self._layers_nccl_fp8(B, L, M, Lpad, packed)
         for i in range(self.n_layers):
             p = f"blocks.{i}."
             check(lib.mmdp_rmsnorm(ptr(x), d, None, ptr(w[p + "attn_norm"]), ptr(xn), d, M, d, self.rms_eps, s))
-            if self.gqa:
+            if packed is not None:
+                self._packed_qkv_attention(p, packed, Lpad)
+            elif self.gqa:
                 check(lib.mmdp_qkv_rope_tp_gqa(ptr(xn), d, ptr(w[p + "wqkv"]), ptr(w.get(p + "bqkv")), M, d, self.h_local, self.kv_local,
                                                L, Lpad, ptr(self.cos), ptr(self.sin), ptr(self.q), ptr(self.k), ptr(self.vt), s))
                 check(lib.mmdp_attention_gqa(ptr(self.q), ptr(self.k), ptr(self.vt), ptr(self.att), B, None, self.h_local, self.kv_local,
@@ -371,7 +409,7 @@ class TensorParallelLLaDA:
             self._allreduce(self.part[:M])
             check(lib.mmdp_resid_add_f32(ptr(x), d, ptr(self.part), d, M, d, s))
 
-    def _layers_nccl_fp8(self, B: int, L: int, M: int, Lpad: int):
+    def _layers_nccl_fp8(self, B: int, L: int, M: int, Lpad: int, packed=None):
         """_layers_nccl with the four linears in FP8: each bf16 input is quantised (1 x 128 groups) right before its GEMM."""
         d, s, w, da, ffl = self.d_model, stream_ptr(), self.w, self.d_attn, self.ff_local
         scale = 1.0 / math.sqrt(128.0)
@@ -380,13 +418,16 @@ class TensorParallelLLaDA:
             p = f"blocks.{i}."
             check(lib.mmdp_rmsnorm(ptr(x), d, None, ptr(w[p + "attn_norm"]), ptr(xn), d, M, d, self.rms_eps, s))
             self._quantize_input(xn, M, d, s)
-            check(lib.mmdp_qkv_rope_tp_fp8(a8, d, a8s, ptr(w[p + "wqkv8"]), ptr(w[p + "sqkv"]), ptr(w.get(p + "bqkv")), M, d, self.h_local,
-                                           self.kv_local, L, Lpad, ptr(self.cos), ptr(self.sin), ptr(self.q), ptr(self.k), ptr(self.vt), s))
-            if self.gqa:
-                check(lib.mmdp_attention_gqa(ptr(self.q), ptr(self.k), ptr(self.vt), ptr(self.att), B, None, self.h_local, self.kv_local,
-                                             L, Lpad, scale, s))
+            if packed is not None:
+                self._packed_qkv_attention(p, packed, Lpad, a8, a8s)
             else:
-                check(lib.mmdp_attention(ptr(self.q), ptr(self.k), ptr(self.vt), ptr(self.att), B, self.h_local, L, Lpad, scale, s))
+                check(lib.mmdp_qkv_rope_tp_fp8(a8, d, a8s, ptr(w[p + "wqkv8"]), ptr(w[p + "sqkv"]), ptr(w.get(p + "bqkv")), M, d, self.h_local,
+                                               self.kv_local, L, Lpad, ptr(self.cos), ptr(self.sin), ptr(self.q), ptr(self.k), ptr(self.vt), s))
+                if self.gqa:
+                    check(lib.mmdp_attention_gqa(ptr(self.q), ptr(self.k), ptr(self.vt), ptr(self.att), B, None, self.h_local, self.kv_local,
+                                                 L, Lpad, scale, s))
+                else:
+                    check(lib.mmdp_attention(ptr(self.q), ptr(self.k), ptr(self.vt), ptr(self.att), B, self.h_local, L, Lpad, scale, s))
             self._quantize_input(self.att, M, da, s)
             check(lib.mmdp_gemm_fp8_f32(a8, da, a8s, ptr(w[p + "wo8"]), da, ptr(w[p + "so"]), M, d, da, ptr(self.part), d, s))
             self._allreduce(self.part[:M])
@@ -405,6 +446,14 @@ class TensorParallelLLaDA:
         key = (B, L)
         if getattr(self, "_ctx_key", None) == key:
             return self._ctx
+        split = chunk_split(B * L) if self.chunks == 2 else [B * L]
+        self._ctx, self._ctx_layers = self._make_ctx(self.vt, split)
+        self._ctx_key = key
+        return self._ctx
+
+    def _make_ctx(self, vt: torch.Tensor, split: List[int]):
+        """mmdp_tp_ctx of this rank over the V^T buffer `vt` and the row chunks `split`; returns it with the layer arrays it points
+        to (the caller keeps them alive)."""
         w = self.w
         layers = (_lib.TpLayer * self.n_layers)()
         fp8 = self.precision == "fp8"
@@ -427,7 +476,7 @@ class TensorParallelLLaDA:
         c.layers = layers
         c.wte, c.ln_f, c.vocab = w["wte"].data_ptr(), w["ln_f"].data_ptr(), w["wte"].shape[0]
         c.cos_tab, c.sin_tab = self.cos.data_ptr(), self.sin.data_ptr()
-        c.q, c.k, c.att, c.h, c.vt = self.q.data_ptr(), self.k.data_ptr(), self.att.data_ptr(), self.h.data_ptr(), self.vt.data_ptr()
+        c.q, c.k, c.att, c.h, c.vt = self.q.data_ptr(), self.k.data_ptr(), self.att.data_ptr(), self.h.data_ptr(), vt.data_ptr()
         c.xn = C.cast(self._xn.array, C.POINTER(C.c_void_p))
         if fp8:
             c.precision = _lib.PRECISION_FP8
@@ -435,18 +484,17 @@ class TensorParallelLLaDA:
             c.xq = C.cast(self._xq_arr, C.POINTER(C.c_void_p))
             c.xq_scales = C.cast(self._xs_arr, C.POINTER(C.c_void_p))
             c.a8, c.a8_scales = self.a8.data_ptr(), self.a8s.data_ptr()
-        split = chunk_split(B * L) if self.chunks == 2 else [B * L]
         c.n_chunks = len(split)
         c.chunk_rows0 = split[0]
-        for ci in range(len(split)):
+        c.packed.seg_pos, c.packed.max_rows, c.packed.rope_len = self._row_map.data_ptr(), self.Mmax, self.max_seq_len
+        for ci in range(self._alloc_chunks):  # both chunks' buffers: a packed forward picks its split per call
             st = self._chunk_state[ci]
             c.chunk[ci].x_shard = st["x"].data_ptr()
             c.chunk[ci].recv[0] = C.cast(st["recv"][0].array, C.POINTER(C.c_void_p))
             c.chunk[ci].recv[1] = C.cast(st["recv"][1].array, C.POINTER(C.c_void_p))
             c.chunk[ci].flags = C.cast(st["flags"].array, C.POINTER(C.c_void_p))
             c.chunk[ci].done_counter = st["done"].data_ptr()
-        self._ctx, self._ctx_layers, self._ctx_key = c, (layers, layers8), key   # (keep the layer arrays alive)
-        return c
+        return c, (layers, layers8)
 
     def _final_norm(self, ids: torch.Tensor) -> torch.Tensor:
         """Runs embedding + all blocks; returns ln_f(x) for ALL rows [M, d] (p2p) or the raw residual stream x (nccl)."""
@@ -472,10 +520,74 @@ class TensorParallelLLaDA:
         self._layers_nccl(B, L, M, Lpad)
         return self.x
 
+    def _prepare_packed_vt(self, lens: List[int], Lpad: int) -> None:
+        """V^T pad rule of the packed buffer (csrc/api.cu, vt_prepare): block s is read up to Lpad and its columns [L_s, Lpad) must
+        be zeros. The buffer is zeroed when the column stride changes or when one of the blocks held more columns than its new
+        length; otherwise every column read past L_s is still zero. Packed and equal-length forwards alternate freely: the
+        equal-length forward keeps its own buffer."""
+        if self._pvt is None:
+            rows = self.max_batch * self.kv_local * 128 * ((self.max_seq_len + 7) // 8 * 8)
+            self._pvt = torch.zeros(rows, dtype=torch.bfloat16, device=self.device)
+            if self.collective == "p2p":
+                self._pctx = self._make_ctx(self._pvt, [1])   # built once; the row chunks are set per call
+        if self._pvt_Lpad != Lpad or any(old > new for old, new in zip(self._pvt_len, lens)):
+            self._pvt.zero_()
+            self._pvt_len = [0] * self.max_batch
+            self._pvt_Lpad = Lpad
+        self._pvt_len[:len(lens)] = lens
+
+    def _final_norm_packed(self, ids: torch.Tensor, lens: List[int]) -> torch.Tensor:
+        """_final_norm over a packed batch (lengths already checked): ln_f(x) of all packed rows (p2p) or the raw x (nccl)."""
+        M, d, s = sum(lens), self.d_model, stream_ptr()
+        split = chunk_split(M) if (self.collective == "p2p" and self.chunks == 2) else [M]
+        if self.collective == "p2p":
+            for rows in split:
+                if row_partition(rows, self.tp, self.tp - 1)[1] < 1:
+                    raise ValueError(f"TensorParallelLLaDA: {rows} packed rows cannot be split over {self.tp} ranks with at least one row each")
+        Lpad = (max(lens) + 7) // 8 * 8
+        self._prepare_packed_vt(lens, Lpad)
+        c_lens = (C.c_int32 * len(lens))(*lens)
+        if self.collective == "p2p":
+            c = self._pctx[0]
+            c.n_chunks, c.chunk_rows0 = len(split), split[0]
+            out = C.c_uint32(0)
+            check(lib.mmdp_tp_forward_packed(C.byref(c), ptr(ids), len(lens), c_lens, self._epoch, C.byref(out), s))
+            self._epoch = int(out.value)
+            return self.xn
+        wte = self.w["wte"]
+        check(lib.mmdp_embed(ptr(ids), ptr(wte), ptr(self.x), M, d, wte.shape[0], s))
+        self._layers_nccl(0, 0, M, Lpad, packed=(len(lens), c_lens))
+        return self.x
+
     @torch.no_grad()
     def forward_rows(self, ids: torch.Tensor, rows_a: Optional[torch.Tensor] = None, rows_b: Optional[torch.Tensor] = None,
                      col0_b: int = 0, ncols_b: int = 0, out_a: Optional[torch.Tensor] = None, out_b: Optional[torch.Tensor] = None):
         hid = self._final_norm(ids.contiguous())
+        return self._head(hid, rows_a, rows_b, col0_b, ncols_b, out_a, out_b)
+
+    @torch.no_grad()
+    def forward_rows_packed(self, ids_packed: torch.Tensor, seq_lens, rows_a: Optional[torch.Tensor] = None,
+                            rows_b: Optional[torch.Tensor] = None, col0_b: int = 0, ncols_b: int = 0,
+                            out_a: Optional[torch.Tensor] = None, out_b: Optional[torch.Tensor] = None, row_windows=None):
+        """One forward over a packed batch: ids_packed [sum(seq_lens)] holds the sequences end to end, each computed as if it were
+        alone (attention stays inside it, positions restart at 0), the contract of LLaDAForMultiModalGeneration.forward_rows_packed.
+        rows_* are int32 packed row indices; the LM head is forward_rows'. At most max_batch sequences (and 64), each at most
+        max_seq_len long: ValueError before anything is launched. The tensor-parallel model has no row windows (row_windows must
+        be None)."""
+        if row_windows is not None:
+            raise NotImplementedError("the tensor-parallel model has no last-block row windows")
+        lens = [int(x) for x in seq_lens]
+        if not lens or len(lens) > min(self.max_batch, 64):
+            raise ValueError(f"a packed forward takes 1 to max_batch={self.max_batch} (at most 64) sequences, got {len(lens)}")
+        if min(lens) < 1 or max(lens) > self.max_seq_len:
+            raise ValueError(f"packed sequence lengths must lie in [1, max_seq_len={self.max_seq_len}], got {lens}")
+        if ids_packed.numel() != sum(lens):
+            raise ValueError(f"ids_packed holds {ids_packed.numel()} tokens, the sequence lengths add up to {sum(lens)}")
+        hid = self._final_norm_packed(ids_packed.to(device=self.device, dtype=torch.int64).contiguous(), lens)
+        return self._head(hid, rows_a, rows_b, col0_b, ncols_b, out_a, out_b)
+
+    def _head(self, hid: torch.Tensor, rows_a, rows_b, col0_b: int, ncols_b: int, out_a, out_b):
+        """The LM head on the rows of `hid` (_final_norm's result): vocabulary slices of this rank, all-gathered."""
         d, s, w = self.d_model, stream_ptr(), self.w
 
         def rows_normed(rows):
