@@ -29,6 +29,7 @@ static constexpr int BM = 128, BK = 64;
 static constexpr int kABytes = BM * BK * 2;  // 16 KB
 static constexpr int kGemmThreads = 384;
 static constexpr int kStagedEpiThreads = 96;  // warps 1-3 of the producer warpgroup run the staged epilogue
+static constexpr int kStagedEpiRegs = 88;     // their register budget (setmaxnreg); the MMA warpgroups get the rest
 // The N tile width is a template parameter: 256 (default; required by the QKV/SwiGLU epilogues) or 192. The K loop and
 // therefore the fp32 accumulation order of every output element is identical for both, so results do not depend on
 // the tile width; the host picks the width that minimises (waves x width) for the problem (wave quantisation on the SMs).
@@ -68,13 +69,17 @@ __device__ __forceinline__ void bf16x8_to_float(uint4 x, float (&f)[8]) {
 // at a multiple of 8, the block is transposed in registers and each column (one d of V^T) is one 16-byte store; otherwise
 // (a sequence boundary inside the 8 rows, a position map, rows past M) every row goes through epi_row8's element stores.
 // Grouped-query tiles (EPI_QKVGQA*) pass cg0 = 16 x the tile's rotary halves: only the 8-column groups from cg0 on are V.
+// `nthr` threads (etid < nthr) share the items. x is indexed with constants only, so it stays in registers. Eight consecutive
+// threads take eight column groups of one 8-row group (their 16-byte staging reads fall in 32 distinct banks) and a warp
+// covers four consecutive 8-row groups, so each column store of a warp writes 64 contiguous bytes (two whole sectors) into
+// each of eight V^T rows instead of 16 bytes into each of 32.
 template <int EPI, int BN>
-__device__ __forceinline__ void staged_vt(const GemmParams& p, const uint8_t* stg, int m_blk, int n_blk, int etid, int cg0 = 0) {
+__device__ __forceinline__ void staged_vt(const GemmParams& p, const uint8_t* stg, int m_blk, int n_blk, int etid, int nthr, int cg0 = 0) {
     constexpr int kStride = GemmCfg<BN, true>::kStagingStride;
     const int CG = BN / 8 - cg0;
     const bool aligned = (p.Lpad & 7) == 0 && (reinterpret_cast<uintptr_t>(p.vt) & 15) == 0;
-    for (int idx = etid; idx < 16 * CG; idx += kStagedEpiThreads) {
-        const int rg = idx / CG, cg = cg0 + idx - rg * CG;
+    for (int idx = etid; idx < 16 * CG; idx += nthr) {
+        const int rg = (idx >> 3) & 15, cg = cg0 + (idx & 7) + 8 * (idx >> 7);  // CG is 16 or 32
         const int r0 = m_blk * 128 + 8 * rg;
         if (r0 >= p.M) continue;
         uint4 x[8];
@@ -83,10 +88,14 @@ __device__ __forceinline__ void staged_vt(const GemmParams& p, const uint8_t* st
         int b0, pos0;
         qkv_row_coords<EPI>(p, r0, b0, pos0);
         bool vec = aligned && r0 + 7 < p.M && (pos0 & 7) == 0;
-        for (int i = 1; i < 8 && vec; ++i) {
-            int b, pos;
-            qkv_row_coords<EPI>(p, r0 + i, b, pos);
-            vec = b == b0 && pos == pos0 + i;
+        if (epi_is_packed(EPI) || p.pos_map) {
+            for (int i = 1; i < 8 && vec; ++i) {
+                int b, pos;
+                qkv_row_coords<EPI>(p, r0 + i, b, pos);
+                vec = b == b0 && pos == pos0 + i;
+            }
+        } else {
+            vec = vec && pos0 + 7 < p.L;  // rows r0 + i are positions pos0 + i of one sequence
         }
         if (vec) {
             const int n = n_blk * BN - (epi_is_gqa(EPI) ? p.d_model + p.n_kv_heads * 128 : 2 * p.d_model) + 8 * cg;
@@ -110,62 +119,88 @@ __device__ __forceinline__ void staged_vt(const GemmParams& p, const uint8_t* st
             for (int i = 0; i < 8; ++i) {
                 if (r0 + i >= p.M) break;
                 float v[8];
-                bf16x8_to_float(x[i], v);
+                bf16x8_to_float(x[0], v);
                 epi_row8<EPI, BN>(p, r0 + i, n_blk, 8 * cg, v, v, zero);
+#pragma unroll
+                for (int j = 0; j < 7; ++j) x[j] = x[j + 1];  // row r0 + i + 1 moves to x[0]
             }
         }
     }
 }
 
-// Epilogue warps: the fused epilogue of one staged tile. Items are (row, 8-column group) as in the split-K finishing pass;
-// consecutive threads take consecutive groups of a row, so a warp reads a row's 16-byte chunks (512 contiguous bytes: no
-// bank conflict) and its global loads and stores are whole 16-byte pieces of one or two rows. Plain and residual items run
-// U at a time with all their loads issued before the first store (C may be the residual: the compiler cannot reorder them).
+// The fused epilogue of one staged tile, shared by `nthr` threads (etid < nthr). Items are (row, 8-column group) as in the
+// split-K finishing pass; consecutive threads take consecutive groups of a row, so a warp reads a row's 16-byte chunks (512
+// contiguous bytes: no bank conflict) and its global loads and stores are whole 16-byte pieces of one or two rows. Plain and
+// residual items run U at a time with all their loads issued before the first store (C may be the residual: the compiler
+// cannot reorder them).
 template <int EPI, int BN>
-__device__ __forceinline__ void staged_epilogue(const GemmParams& p, const uint8_t* stg, int m_blk, int n_blk, int etid) {
+__device__ __forceinline__ void staged_epilogue(const GemmParams& p, const uint8_t* stg, int m_blk, int n_blk, int etid, int nthr) {
     constexpr int kStride = GemmCfg<BN, true>::kStagingStride;
-    if constexpr (EPI == EPI_QKVROPE || EPI == EPI_QKVROPE_PACKED) {
-        if (n_blk * BN >= 2 * p.d_model) {
-            staged_vt<EPI, BN>(p, stg, m_blk, n_blk, etid);
-            return;
-        }
-    }
-    // grouped-query tiles: V halves through staged_vt, then the rotary items of the q / k halves (8 per half and row)
-    int n_rot = BN / 128;
-    if constexpr (epi_is_gqa(EPI)) {
-        n_rot = gqa_rot_halves<BN>(p, n_blk);
-        if (n_rot < BN / 128) staged_vt<EPI, BN>(p, stg, m_blk, n_blk, etid, 16 * n_rot);
-    }
-    constexpr bool kPair = EPI == EPI_SWIGLU || epi_is_qkv(EPI);
-    constexpr int G = kPair ? 16 : BN / 8;
-    const int kItems = epi_is_gqa(EPI) ? BM * 8 * n_rot : BM * G;
-    const int Gi = epi_is_gqa(EPI) ? 8 * n_rot : G;
-    constexpr int U = kPair ? 1 : 4;
-    for (int i0 = etid; i0 < kItems; i0 += U * kStagedEpiThreads) {
-        uint4 xv[U], xw[U], rv[U];
-        int row[U], tc[U];
+    if constexpr (epi_is_qkv(EPI)) {
+        int n_rot = BN / 128;  // rotary (q / k) halves of the tile; the rest is V
+        if constexpr (epi_is_gqa(EPI)) n_rot = gqa_rot_halves<BN>(p, n_blk);
+        else if (n_blk * BN >= 2 * p.d_model) n_rot = 0;
+        if (n_rot < BN / 128) staged_vt<EPI, BN>(p, stg, m_blk, n_blk, etid, nthr, 16 * n_rot);
+        if (n_rot == 0) return;
+        // rotary items (row, 8-column group gg) span the tile's rotary halves: columns 128 h + 8 gg and their partners + 64
+        // all take the cos / sin of (position, 8 gg), loaded once. Every load of an item (up to 4 staging chunks, the row's
+        // position, 4 cos / sin chunks) is issued before its first store.
+        for (int idx = etid; idx < BM * 8; idx += nthr) {
+            const int rit = idx >> 3, gg = idx & 7;
+            const int row = m_blk * BM + rit;
+            if (row >= p.M) break;
+            uint4 xv[BN / 128], xw[BN / 128];
 #pragma unroll
-        for (int u = 0; u < U; ++u) {
-            const int idx = i0 + u * kStagedEpiThreads;
-            const int rit = idx / Gi, g = idx - rit * Gi;
-            // SwiGLU g -> gate columns 8g, up +128; rotary g = (head, gg) -> 128 head + 8 gg, partner +64
-            tc[u] = EPI == EPI_SWIGLU ? 8 * g : (kPair ? (g >> 3) * 128 + 8 * (g & 7) : 8 * g);
-            row[u] = (idx < kItems && m_blk * BM + rit < p.M) ? m_blk * BM + rit : -1;
-            rv[u] = make_uint4(0, 0, 0, 0);
-            if (row[u] < 0) continue;
-            xv[u] = *reinterpret_cast<const uint4*>(stg + rit * kStride + tc[u] * 2);
-            if constexpr (kPair) xw[u] = *reinterpret_cast<const uint4*>(stg + rit * kStride + (tc[u] + (EPI == EPI_SWIGLU ? 128 : 64)) * 2);
-            if constexpr (EPI == EPI_RESID) {
-                if (n_blk * BN + tc[u] < p.N) rv[u] = *reinterpret_cast<const uint4*>(p.resid + (size_t)row[u] * p.ldr + n_blk * BN + tc[u]);
+            for (int h = 0; h < BN / 128; ++h) {
+                if (h < n_rot) {
+                    xv[h] = *reinterpret_cast<const uint4*>(stg + rit * kStride + (128 * h + 8 * gg) * 2);
+                    xw[h] = *reinterpret_cast<const uint4*>(stg + rit * kStride + (128 * h + 8 * gg + 64) * 2);
+                }
+            }
+            int sq, pos;
+            qkv_row_coords<EPI>(p, row, sq, pos);
+            float4 cs[2], sn[2];
+            rope_cs_load(p, pos, 8 * gg, cs, sn);
+#pragma unroll
+            for (int h = 0; h < BN / 128; ++h) {
+                if (h < n_rot) {
+                    float v[8], w[8];
+                    bf16x8_to_float(xv[h], v);
+                    bf16x8_to_float(xw[h], w);
+                    qkv_rope_item<EPI, BN>(p, row, sq, pos, n_blk, 128 * h + 8 * gg, v, w, cs, sn);
+                }
             }
         }
+    } else {
+        constexpr bool kPair = EPI == EPI_SWIGLU;
+        constexpr int G = kPair ? 16 : BN / 8;
+        constexpr int kItems = BM * G;
+        constexpr int U = kPair ? 1 : 4;
+        for (int i0 = etid; i0 < kItems; i0 += U * nthr) {
+            uint4 xv[U], xw[U], rv[U];
+            int row[U], tc[U];
 #pragma unroll
-        for (int u = 0; u < U; ++u) {
-            if (row[u] < 0) continue;
-            float v[8], w[8];
-            bf16x8_to_float(xv[u], v);
-            if constexpr (kPair) bf16x8_to_float(xw[u], w);
-            epi_row8<EPI, BN>(p, row[u], n_blk, tc[u], v, kPair ? w : v, rv[u]);
+            for (int u = 0; u < U; ++u) {
+                const int idx = i0 + u * nthr;
+                const int rit = idx / G, g = idx - rit * G;
+                tc[u] = 8 * g;  // SwiGLU: gate columns 8g, up + 128
+                row[u] = (idx < kItems && m_blk * BM + rit < p.M) ? m_blk * BM + rit : -1;
+                rv[u] = make_uint4(0, 0, 0, 0);
+                if (row[u] < 0) continue;
+                xv[u] = *reinterpret_cast<const uint4*>(stg + rit * kStride + tc[u] * 2);
+                if constexpr (kPair) xw[u] = *reinterpret_cast<const uint4*>(stg + rit * kStride + (tc[u] + 128) * 2);
+                if constexpr (EPI == EPI_RESID) {
+                    if (n_blk * BN + tc[u] < p.N) rv[u] = *reinterpret_cast<const uint4*>(p.resid + (size_t)row[u] * p.ldr + n_blk * BN + tc[u]);
+                }
+            }
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                if (row[u] < 0) continue;
+                float v[8], w[8];
+                bf16x8_to_float(xv[u], v);
+                if constexpr (kPair) bf16x8_to_float(xw[u], w);
+                epi_row8<EPI, BN>(p, row[u], n_blk, tc[u], v, kPair ? w : v, rv[u]);
+            }
         }
     }
 }
@@ -225,8 +260,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
     if (wg == 0) {
         // ===================== TMA producer (warp 0) and staged epilogue (warps 1-3) =====================
-        // 56 / 224 / 224 registers per thread: 64 512 of the 65 536 for 384 threads
-        setmaxnreg_dec<kStaged ? 56 : 40>();
+        // staged: 88 / 208 / 208 registers per thread (64 512 of the 65 536 for 384 threads): the epilogue warps keep a
+        // rotary item's loads (4 staging chunks, 4 cos / sin chunks) and V^T's 8 x 8 block in registers without spilling
+        setmaxnreg_dec<kStaged ? kStagedEpiRegs : 40>();
         if constexpr (kStaged) {
             if (warp > 0) {
                 const int etid = threadIdx.x - 32;
@@ -235,7 +271,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     int m_blk, n_blk;
                     gemm_tile_coords(tile, num_m, num_n, p.group_m, m_blk, n_blk);
                     mbar_wait(staged_bar, it & 1);
-                    staged_epilogue<EPI, BN>(p, staging, m_blk, n_blk, etid);
+                    const bool shared = !has_unit && tile + (int)gridDim.x >= full_tiles;  // the MMA warps join (below)
+                    staged_epilogue<EPI, BN>(p, staging, m_blk, n_blk, etid, shared ? kStagedEpiThreads + 256 : kStagedEpiThreads);
                     mbar_arrive(drained_bar);
                 }
             }
@@ -267,7 +304,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         __syncwarp();
     } else {
         // ===================== MMA + epilogue (warpgroups 1 and 2: tile rows [64 (wg-1), 64 wg)) =====================
-        setmaxnreg_inc<kStaged ? 224 : 232>();
+        setmaxnreg_inc<kStaged ? (64512 - 128 * kStagedEpiRegs) / 256 : 232>();
         const int half = wg - 1;
         const int rit0 = half * 64 + (warp & 3) * 16 + (lane >> 2);  // tile row of acc[4j + 0..1]; acc[4j + 2..3] is 8 rows below
         const int c0 = 2 * (lane & 3);
@@ -275,6 +312,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         int s = 0;
         uint32_t ph = 0;
         uint32_t it = 0;  // full tiles staged so far
+        int last_m = -1, last_n = 0;  // the last staged tile
         for (int tile = blockIdx.x; tile < full_tiles + (has_unit ? 1 : 0) * gridDim.x; tile += gridDim.x) {
             const bool is_unit = tile >= full_tiles;
             const int tl = is_unit ? unit_tile : tile;
@@ -354,8 +392,17 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 stage_tile<BN>(staging, acc, rit0, c0);
                 mbar_arrive(staged_bar);
                 ++it;
+                last_m = m_blk; last_n = n_blk;
             } else {
                 gemm_epilogue_tile<EPI, BN>(p, acc, m_blk, n_blk, rit0, c0);
+            }
+        }
+        if constexpr (kStaged) {
+            // this CTA's last tile has no main loop left to hide its epilogue under: the MMA warps drain it together with the
+            // epilogue warps once every staging store has landed (a CTA with a split-K unit hides it under the unit instead)
+            if (!has_unit && last_m >= 0) {
+                mbar_wait(staged_bar, (it - 1) & 1);
+                staged_epilogue<EPI, BN>(p, staging, last_m, last_n, kStagedEpiThreads + threadIdx.x - 128, kStagedEpiThreads + 256);
             }
         }
         if constexpr (EPI == EPI_F32) {

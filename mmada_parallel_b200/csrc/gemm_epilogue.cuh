@@ -323,6 +323,38 @@ __device__ __forceinline__ void sk_publish(float* __restrict__ slot_ws, const fl
         }
 }
 
+// cos / sin of position `pos`, table columns c .. c + 7 (the rotary item's angles)
+__device__ __forceinline__ void rope_cs_load(const GemmParams& p, int pos, int c, float4 (&cs)[2], float4 (&sn)[2]) {
+    const float4* c4 = reinterpret_cast<const float4*>(p.cos_tab + (size_t)pos * 64 + c);
+    const float4* s4 = reinterpret_cast<const float4*>(p.sin_tab + (size_t)pos * 64 + c);
+    cs[0] = c4[0]; cs[1] = c4[1]; sn[0] = s4[0]; sn[1] = s4[1];
+}
+
+// Rotary item of the QKV epilogues: q / k columns tc .. tc + 7 (v) and their partners tc + 64 .. (w) of GEMM row `row`
+// (sequence b, position pos), with that position's cos / sin already loaded; stores 2 x 8 bf16.
+template <int EPI, int BN>
+__device__ __forceinline__ void qkv_rope_item(const GemmParams& p, int row, int b, int pos, int n_blk, int tc, const float (&v)[8],
+                                              const float (&w)[8], const float4 (&cs4)[2], const float4 (&sn4)[2]) {
+    const int n0 = n_blk * BN;
+    const float cs[8] = {cs4[0].x, cs4[0].y, cs4[0].z, cs4[0].w, cs4[1].x, cs4[1].y, cs4[1].z, cs4[1].w};
+    const float sn[8] = {sn4[0].x, sn4[0].y, sn4[0].z, sn4[0].w, sn4[1].x, sn4[1].y, sn4[1].z, sn4[1].w};
+    float o1[8], o2[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) rope_pair(bf16_round(v[i]), bf16_round(w[i]), cs[i], sn[i], o1[i], o2[i]);
+    __nv_bfloat16* dst;
+    if constexpr (epi_is_gqa(EPI)) {
+        dst = gqa_qk_dst(p, row, n0 + tc);
+    } else {
+        const int region = n0 / p.d_model;  // 0 = Q, 1 = K (d_model % 256 == 0 is checked on the host)
+        const size_t drow = (region == 0 || !p.pos_map) ? (size_t)row : (size_t)b * p.L + pos;  // k rows go to their sequence position
+        dst = (region == 0 ? p.q : p.k) + drow * p.d_model + (n0 - region * p.d_model) + (tc >> 7) * 128 + (tc & 63);
+    }
+    *reinterpret_cast<uint4*>(dst) =
+        make_uint4(pack_bf16x2(o1[0], o1[1]), pack_bf16x2(o1[2], o1[3]), pack_bf16x2(o1[4], o1[5]), pack_bf16x2(o1[6], o1[7]));
+    *reinterpret_cast<uint4*>(dst + 64) =
+        make_uint4(pack_bf16x2(o2[0], o2[1]), pack_bf16x2(o2[2], o2[3]), pack_bf16x2(o2[4], o2[5]), pack_bf16x2(o2[6], o2[7]));
+}
+
 // One work item of the fused epilogue, shared by the split-K finishing pass (fp32 sums) and the staged epilogue of
 // gemm_bf16_kernel (bf16 values from shared memory; every epilogue rounds the accumulator to bf16 first, so both give the
 // same bits as gemm_epilogue_tile): output row `row` (< p.M), 8 consecutive tile columns from `tc`, values v. The rotary and
@@ -370,26 +402,9 @@ __device__ __forceinline__ void epi_row8(const GemmParams& p, int row, int n_blk
         int b, pos;
         qkv_row_coords<EPI>(p, row, b, pos);
         if (region < 2) {
-            const int head = tc >> 7, c = tc & 63;  // tc = head * 128 + c, c < 64
-            const float4* c4 = reinterpret_cast<const float4*>(p.cos_tab + (size_t)pos * 64 + c);
-            const float4* s4 = reinterpret_cast<const float4*>(p.sin_tab + (size_t)pos * 64 + c);
-            const float4 c0 = c4[0], c1 = c4[1], s0 = s4[0], s1 = s4[1];
-            const float cs[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
-            const float sn[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-            float o1[8], o2[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const float t1 = bf16_round(v[i]), t2 = bf16_round(w[i]);
-                // (t * cos) + (rotate_half(t) * sin), fp32, no FMA contraction
-                o1[i] = __fadd_rn(__fmul_rn(t1, cs[i]), __fmul_rn(-t2, sn[i]));
-                o2[i] = __fadd_rn(__fmul_rn(t2, cs[i]), __fmul_rn(t1, sn[i]));
-            }
-            const size_t drow = (region == 0 || !p.pos_map) ? (size_t)row : (size_t)b * p.L + pos;  // k rows go to their sequence position
-            __nv_bfloat16* dst = (region == 0 ? p.q : p.k) + drow * p.d_model + (n0 - region * p.d_model) + head * 128 + c;
-            *reinterpret_cast<uint4*>(dst) =
-                make_uint4(pack_bf16x2(o1[0], o1[1]), pack_bf16x2(o1[2], o1[3]), pack_bf16x2(o1[4], o1[5]), pack_bf16x2(o1[6], o1[7]));
-            *reinterpret_cast<uint4*>(dst + 64) =
-                make_uint4(pack_bf16x2(o2[0], o2[1]), pack_bf16x2(o2[2], o2[3]), pack_bf16x2(o2[4], o2[5]), pack_bf16x2(o2[6], o2[7]));
+            float4 cs[2], sn[2];
+            rope_cs_load(p, pos, tc & 63, cs, sn);  // tc = head * 128 + c, c < 64
+            qkv_rope_item<EPI, BN>(p, row, b, pos, n_blk, tc, v, w, cs, sn);
         } else {
             // V is written transposed: vt[b][head][d][token] so that P·V runs with both operands K-major
             const int n = n0 - 2 * p.d_model + tc;
@@ -404,20 +419,9 @@ __device__ __forceinline__ void epi_row8(const GemmParams& p, int row, int n_blk
         qkv_row_coords<EPI>(p, row, b, pos);
         const int col = n0 + tc;
         if (col < p.d_model + p.n_kv_heads * 128) {
-            const int c = tc & 63;
-            const float4* c4 = reinterpret_cast<const float4*>(p.cos_tab + (size_t)pos * 64 + c);
-            const float4* s4 = reinterpret_cast<const float4*>(p.sin_tab + (size_t)pos * 64 + c);
-            const float4 c0 = c4[0], c1 = c4[1], s0 = s4[0], s1 = s4[1];
-            const float cs[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
-            const float sn[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-            float o1[8], o2[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) rope_pair(bf16_round(v[i]), bf16_round(w[i]), cs[i], sn[i], o1[i], o2[i]);
-            __nv_bfloat16* dst = gqa_qk_dst(p, row, col);
-            *reinterpret_cast<uint4*>(dst) =
-                make_uint4(pack_bf16x2(o1[0], o1[1]), pack_bf16x2(o1[2], o1[3]), pack_bf16x2(o1[4], o1[5]), pack_bf16x2(o1[6], o1[7]));
-            *reinterpret_cast<uint4*>(dst + 64) =
-                make_uint4(pack_bf16x2(o2[0], o2[1]), pack_bf16x2(o2[2], o2[3]), pack_bf16x2(o2[4], o2[5]), pack_bf16x2(o2[6], o2[7]));
+            float4 cs[2], sn[2];
+            rope_cs_load(p, pos, tc & 63, cs, sn);
+            qkv_rope_item<EPI, BN>(p, row, b, pos, n_blk, tc, v, w, cs, sn);
         } else {
             __nv_bfloat16* dst = gqa_vt_dst(p, col, b, pos);
 #pragma unroll

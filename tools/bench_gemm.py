@@ -7,7 +7,7 @@ in the same run (nvidia-smi query).
 Per-tile fixed cost: with the split-K tail off every CTA runs whole tiles, so a launch takes t(K) = waves * (K/64 * c + x),
 where c is the main-loop time of one 64-deep k-block and x what a tile costs beyond its main loop (the epilogue and whatever
 the pipeline cannot hide at a tile boundary). Timing the same M x N at K = 4096 and K = 12288 gives
-x = (3 * t(4096) - t(12288)) / (2 * waves).
+x = (3 * t(4096) - t(12288)) / (2 * waves). QKV + RoPE takes the same fit: N = 12288 (32 heads) at both K.
 """
 from __future__ import annotations
 
@@ -79,7 +79,17 @@ def main():
     launches = {}
     with torch.no_grad():
         M = L_SAMPLE
-        launches["qkv_rope"] = entry(M, 3 * d, d, time_op(lambda: _lib.qkv_rope(xa[d][:M], w(3 * d, d), H, M, cos, sin), args.reps))
+        # q, k and V^T are allocated once (the forward's buffers are too), so only the GEMM launch is timed
+        q = torch.empty(M, d, dtype=torch.bfloat16, device=device)
+        k = torch.empty_like(q)
+        vt = torch.zeros(1, H, 128, -(-M // 8) * 8, dtype=torch.bfloat16, device=device)
+
+        def qkv(K):
+            """QKV + RoPE of H heads (N = 3 * 128 H) over K input columns: the tensor-parallel entry takes K apart from H."""
+            _lib.check(_lib.lib.mmdp_qkv_rope_tp(_lib.ptr(xa[K]), K, _lib.ptr(w(3 * d, K)), M, K, H, M, vt.shape[-1], _lib.ptr(cos),
+                                                 _lib.ptr(sin), _lib.ptr(q), _lib.ptr(k), _lib.ptr(vt), _lib.stream_ptr()))
+
+        launches["qkv_rope"] = entry(M, 3 * d, d, time_op(lambda: qkv(d), args.reps))
         for m in (M,) + WINDOW_M:
             sfx = "" if m == M else f"_m{m}"
             r = resid[:m]
@@ -95,11 +105,15 @@ def main():
         per_tile = {}
         _lib.lib.mmdp_set_gemm_splitk(0)
         try:
-            for name, N, epi in (("plain", 3 * d, _lib.EPI_PLAIN), ("resid", d, _lib.EPI_RESID), ("swiglu", 2 * ff, _lib.EPI_SWIGLU)):
+            for name, N, epi in (("plain", 3 * d, _lib.EPI_PLAIN), ("resid", d, _lib.EPI_RESID), ("swiglu", 2 * ff, _lib.EPI_SWIGLU),
+                                 ("qkv_rope", 3 * d, None)):
                 t = {}
                 for K in (d, ff):
                     r = resid[:M] if epi == _lib.EPI_RESID else None
-                    t[K] = time_op(lambda: _lib.gemm_bf16(xa[K][:M], w(N, K), epi, resid=r, out=r), args.reps)
+                    if epi is None:
+                        t[K] = time_op(lambda: qkv(K), args.reps)
+                    else:
+                        t[K] = time_op(lambda: _lib.gemm_bf16(xa[K][:M], w(N, K), epi, resid=r, out=r), args.reps)
                 waves = waves_no_split(M, N, epi, sms)
                 x_ms = (3 * t[d] - t[ff]) / (2 * waves)
                 loop_ms = t[d] / waves - x_ms  # main loop of one K = 4096 tile
