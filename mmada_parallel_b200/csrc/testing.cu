@@ -1,6 +1,8 @@
-// Test hooks (include/mmdp_testing.h): the internal VQ kernels behind thin C wrappers, so that tests can check each
-// operation against a high-precision restatement of it. Each hook forwards its arguments unchanged.
+// Test hooks (include/mmdp_testing.h: the VQ kernels; include/mmdp_testing_cache.h: the token-cache launches): internal kernels
+// behind thin C wrappers, so that tests can check each operation against a high-precision restatement of it. Each hook forwards
+// its arguments unchanged.
 #include "../../include/mmdp_testing.h"
+#include "../../include/mmdp_testing_cache.h"
 #include "mmdp_internal.h"
 
 using namespace mmdp;
@@ -74,6 +76,30 @@ MMDP_API int mmdp_testing_codebook_to_padded(const int64_t* ids, const float* cb
                                              int64_t n_codes, int* err, void* stream) {
     if (need_device(__func__)) return -1;
     return codebook_to_padded(ids, cb, z, B, h, w, C, Cpad, n_codes, err, (cudaStream_t)stream);
+}
+
+MMDP_API int mmdp_testing_qkv_rope_cached(int precision, const void* A, int lda, const float* sa, const void* Wqkv, const float* sw,
+                                          int B, int Tq, const int32_t* pos_map, int d_model, int n_heads, int L, int Lpad,
+                                          const float* cos, const float* sin, uint16_t* q, uint16_t* kcache, uint16_t* vtcache,
+                                          void* stream) {
+    if (need_device(__func__)) return -1;
+    QkvRopeArgs qa{(__nv_bfloat16*)q, (__nv_bfloat16*)kcache, (__nv_bfloat16*)vtcache, cos, sin, L, Lpad, d_model, n_heads,
+                   pos_map, pos_map ? Tq : 0};
+    const int M = B * Tq, N = 3 * d_model;
+    if (precision == 0)
+        return gemm_bf16(EPI_QKVROPE, (const __nv_bfloat16*)A, lda, (const __nv_bfloat16*)Wqkv, d_model, M, N, d_model, nullptr, 0,
+                         nullptr, 0, &qa, (cudaStream_t)stream);
+    if (precision == 1)
+        return gemm_fp8(EPI_QKVROPE, (const uint8_t*)A, lda, sa, (const uint8_t*)Wqkv, d_model, sw, M, N, d_model, nullptr, 0, nullptr,
+                        0, &qa, (cudaStream_t)stream);
+    return set_error("%s: precision %d is neither 0 (bf16) nor 1 (e4m3)", __func__, precision);
+}
+
+MMDP_API int mmdp_testing_attention_cached(const uint16_t* q, const uint16_t* k, const uint16_t* vt, uint16_t* out, int B, int H,
+                                           int L, int Lpad, int Tq, float scale, void* stream) {
+    if (need_device(__func__)) return -1;
+    return attention_fwd((const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)vt, (__nv_bfloat16*)out, B, H, L, Lpad,
+                         scale, (cudaStream_t)stream, Tq);
 }
 
 }  // extern "C"

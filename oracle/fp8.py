@@ -3,9 +3,9 @@
 The reference has no FP8; these functions ARE the contract the CUDA path (csrc/fp8.cu, include/mmdp.h) is pinned to:
   quantize_fp8   s = amax|x| / 448 per row group (fp32, IEEE division; 1 for an all-zero group), q = e4m3(x / s)
   linear_fp8     acc[m, n] = sw[n] * sum_g sa[g, m] * (sum_{k in g} qa[m, k] * qw[n, k]) in fp32, groups of 128 along K
-  block_forward_fp8 / forward_logits_fp8
-                 oracle.llada's block and forward with the four linears (q/k/v_proj, attn_out, ff_proj/up_proj, ff_out)
-                 replaced by bf16(linear_fp8(quantised input, quantised weight)); weights use one scale per row (group = K),
+  block_forward_fp8 / forward_logits_fp8 / linear_hook
+                 oracle.llada's block, forward and token-cache forward (CachedOracleModel) with the four linears
+                 (q/k/v_proj, attn_out, ff_proj/up_proj, ff_out) replaced by bf16(linear_fp8(quantised input, quantised weight)); weights use one scale per row (group = K),
                  activations 1 x 128 groups. Every other op and bf16 rounding point is oracle.llada's.
 Runs on whatever device its inputs live on (the tests use the CPU, and torch on the GPU for the large shapes).
 """
@@ -65,6 +65,11 @@ def _linear(x: torch.Tensor, qw_sw) -> torch.Tensor:
     qa, sa = quantize_fp8(x.reshape(-1, shape[-1]), ACT_GROUP)
     y = linear_fp8(qa, sa, *qw_sw).to(torch.bfloat16)
     return y.reshape(*shape[:-1], y.shape[-1])
+
+
+def linear_hook(wq: Dict[str, tuple]):
+    """llada.CachedOracleModel's `linear` with the block linears in FP8 (wq = quantize_weights(w))."""
+    return lambda x, name: _linear(x, wq[name])
 
 
 def block_forward_fp8(x: torch.Tensor, w: Dict[str, torch.Tensor], wq: Dict[str, tuple], prefix: str, cfg, pos_sin, pos_cos):

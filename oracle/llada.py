@@ -144,10 +144,14 @@ class CachedOracleModel:
     cat=key) after model.caching(True) - modeling_llada.py:1244-1245 (ids restricted to the masked tokens), :929-940 (per-block
     k / v caches: stored whole without a mask, scattered at the masked positions with one), :715-716 + :412-435 (rotary with the
     masked tokens' own positions for q, all positions for the cached k), :1406-1413 (logit cache; the cache tensor is what is
-    returned). Pinned against the real reference in oracle/make_golden_cache.py."""
+    returned). Pinned against the real reference in oracle/make_golden_cache.py.
+    `linear(x, name)` computes the block linear whose weight is the state-dict entry `name` (q/k/v_proj, attn_out, ff_proj,
+    up_proj, ff_out of a block; not the LM head). Default: F.linear in the weights' dtype, the reference's linear;
+    oracle.fp8.linear_hook gives the FP8 block linears. Runs on the device its weights live on."""
 
-    def __init__(self, cfg, weights: Dict[str, torch.Tensor]):
+    def __init__(self, cfg, weights: Dict[str, torch.Tensor], linear=None):
         self.config, self.w = cfg, weights
+        self.linear = linear if linear is not None else (lambda x, name: F.linear(x, weights[name]))
         self.k, self.v, self.logit = {}, {}, {}
 
     def empty_cache(self):
@@ -163,16 +167,17 @@ class CachedOracleModel:
             ids = ids[to_compute_mask].view(B, -1)                                              # :1244-1245
         x = F.embedding(ids, w["model.transformer.wte.weight"])
         nh, C = cfg.n_heads, cfg.d_model
-        pos_sin, pos_cos = rotary_tables(C // nh, cfg.rope_theta, L)
+        pos_sin, pos_cos = (t.to(x.device) for t in rotary_tables(C // nh, cfg.rope_theta, L))
+        lin = self.linear
         for i in range(cfg.n_layers):
             p = f"model.transformer.blocks.{i}."
             T = x.shape[1]
             xn = rms_norm(x, w[p + "attn_norm.weight"], cfg.rms_norm_eps)
-            q, k, v = (F.linear(xn, w[p + n + ".weight"]) for n in ("q_proj", "k_proj", "v_proj"))
+            q, k, v = (lin(xn, p + n + ".weight") for n in ("q_proj", "k_proj", "v_proj"))
             key = (i, cat)
             if key not in self.k:                                                               # :930-932
-                self.k[key] = torch.zeros(B, L, C, dtype=x.dtype)
-                self.v[key] = torch.zeros(B, L, C, dtype=x.dtype)
+                self.k[key] = torch.zeros(B, L, C, dtype=x.dtype, device=x.device)
+                self.v[key] = torch.zeros(B, L, C, dtype=x.dtype, device=x.device)
             if to_compute_mask is not None:                                                     # :933-937
                 self.k[key][to_compute_mask] = k.reshape(-1, C)
                 self.v[key][to_compute_mask] = v.reshape(-1, C)
@@ -190,10 +195,10 @@ class CachedOracleModel:
             k_ = apply_rotary(pos_sin, pos_cos, kh.float()).type_as(kh)
             att = F.scaled_dot_product_attention(q_, k_, vh, attn_mask=None, dropout_p=0.0, is_causal=False)
             att = att.transpose(1, 2).contiguous().view(B, T, C)
-            x = x + F.linear(att, w[p + "attn_out.weight"])
+            x = x + lin(att, p + "attn_out.weight")
             h = rms_norm(x, w[p + "ff_norm.weight"], cfg.rms_norm_eps)
-            h = F.silu(F.linear(h, w[p + "ff_proj.weight"])) * F.linear(h, w[p + "up_proj.weight"])
-            x = x + F.linear(h, w[p + "ff_out.weight"])
+            h = F.silu(lin(h, p + "ff_proj.weight")) * lin(h, p + "up_proj.weight")
+            x = x + lin(h, p + "ff_out.weight")
         x = rms_norm(x, w["model.transformer.ln_f.weight"], cfg.rms_norm_eps)
         logits = F.linear(x, w["model.transformer.ff_out.weight"])
         if cat not in self.logit:                                                               # :1406-1413

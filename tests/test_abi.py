@@ -80,3 +80,23 @@ def test_testing_hooks_exported_and_fail_without_gpu():
         zeros = [0.0 if a is C.c_float else None if a is C.c_void_p else 1 for a in args]
         assert getattr(lib, n)(*zeros) == -1, n
         assert b"no CUDA device" in _lib.lib.mmdp_last_error(), n
+
+
+def test_token_cache_hooks_exported_and_fail_without_gpu():
+    """Every hook of include/mmdp_testing_cache.h is exported, kept out of the product table and the VQ hook header, and errors
+    (not crashes) without a device."""
+    from mmada_parallel_b200 import _lib
+    from test_gpu_token_cache import HOOKS, declared_cache_symbols, hooks
+    from test_gpu_vq_ops import declared_testing_symbols
+    names = declared_cache_symbols()
+    assert names == sorted(HOOKS) == ["mmdp_testing_attention_cached", "mmdp_testing_qkv_rope_cached"]
+    assert not set(names) & set(declared_testing_symbols())
+    lib = hooks()
+    for n in names:
+        assert n not in _lib.SIGNATURES
+    if torch.cuda.is_available():
+        return
+    for n, args in HOOKS.items():
+        zeros = [0.0 if a is C.c_float else None if a is C.c_void_p else 1 for a in args]
+        assert getattr(lib, n)(*zeros) == -1, n
+        assert b"no CUDA device" in _lib.lib.mmdp_last_error(), n

@@ -4,6 +4,7 @@ of the scheme, not a parity claim)."""
 import math
 
 import torch
+import torch.nn.functional as F
 
 from helpers import load_golden, tiny_cfg_and_weights
 from oracle import fp8, llada
@@ -123,3 +124,26 @@ def test_tiny_forward_fp8_vs_bf16_oracle():
     # model carries that through 2 blocks and 8 linears to ~10 % (measured); a scheme error (wrong scale, lost group) is far larger
     assert rel_rms < 0.25 and rel_max < 0.5
     assert math.isfinite(rel_rms)
+
+
+def test_cached_oracle_linear_hook():
+    """llada.CachedOracleModel's `linear` hook: its default is the reference's bf16 F.linear (the same bits as the hook spelled out,
+    and as the real reference on the token-cache golden's calls), and with fp8.linear_hook the full forward is
+    fp8.forward_logits_fp8 bit for bit, as is a partial forward that recomputes every position."""
+    g = load_golden("forward_tiny.pt")
+    cfg, sd = tiny_cfg_and_weights(g["meta"])
+    t = load_golden("token_cache_tiny.pt")
+    default = llada.CachedOracleModel(cfg, sd)
+    spelled = llada.CachedOracleModel(cfg, sd, linear=lambda x, name: F.linear(x, sd[name]))
+    for case in t["cases"]:
+        for st in case["steps"]:
+            a = default(st["ids"], to_compute_mask=st["mask"], cat=case["cat"]).logits
+            b = spelled(st["ids"], to_compute_mask=st["mask"], cat=case["cat"]).logits
+            assert torch.equal(a, b) and torch.equal(a[:, :, st["cols"]], st["logits_cols"]), case["name"]
+    wq = fp8.quantize_weights(sd)
+    om = llada.CachedOracleModel(cfg, sd, linear=fp8.linear_hook(wq))
+    ids = g["ids"]
+    with torch.no_grad():
+        want = fp8.forward_logits_fp8(ids, sd, cfg, wq)
+    assert torch.equal(om(ids, cat="x").logits, want)
+    assert torch.equal(om(ids, to_compute_mask=torch.ones_like(ids, dtype=torch.bool), cat="x").logits, want)
